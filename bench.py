@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — depth-frames/s (and Mvoxel-updates/s) of the semantic TSDF integrator hot path.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload fast5|merged2|fast10] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload fast5|merged2|fast10] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one synthetic 640x480 depth+label frame (BASELINE.json
 configs[1] by default: 5 cm voxels, 21 classes, `fast` integrator).  Every step integrates a DIFFERENT
@@ -16,6 +16,8 @@ region; for `value` they are already resident in HBM).  One JSON line is printed
   cpu_baseline  the reference's CPU path timed on this box's host cores: the faster of (a) the oracle port and (b) the reference's
             own integrator sources built against stand-in dependency headers (oracle/_ref), each at its best thread count
   --impl reference   times that CPU path alone and prints the same line shape
+  --dump-outputs DIR  after the timed steps, writes the map the timed integrator holds (what ksg_export_blocks hands a caller) as
+            DIR/<name>.npy in float32 / float64, blocks sorted by index; see dump_outputs() for the seeded sample that keeps it under 64 MB
 
 Multi-GPU (torchrun, one rank per GPU): the path shards by sequence - every rank integrates its own camera
 stream into its own map (independent robots / sequences), no data-path collective; "scaling": "weak".
@@ -44,7 +46,9 @@ WORKLOADS = {
     "merged5": (KSG_INTEGRATOR_MERGED, 640, 480, 0.05, 21, 16 << 20, 8192),
     "fast10": (KSG_INTEGRATOR_FAST, 320, 240, 0.10, 5, 0, 4096),        # configs[0] geometry
     "fast5_720p_c150": (KSG_INTEGRATOR_FAST, 1280, 720, 0.05, 150, 0, 2048),   # configs[3]: ADE20K-size label set, frame-per-GPU batches
-    "merged1_4k_c40": (KSG_INTEGRATOR_MERGED, 3840, 2160, 0.01, 40, 1500 << 20, 65536),   # configs[4]: 4K / 1 cm, spatially sharded
+    # configs[4]: 4K / 1 cm, spatially sharded.  Every rank allocates the whole map: 24576 blocks of 40 classes (~18 GB) + 1.5 G records
+    # (~25 GB) fit an 80 GB H100
+    "merged1_4k_c40": (KSG_INTEGRATOR_MERGED, 3840, 2160, 0.01, 40, 1500 << 20, 24576),
 }
 
 
@@ -197,30 +201,6 @@ def best_cpu_arm(workload, frames, cam):
     return best[0], best[1], {f"{a}@{t}": v for (a, t), v in res.items()}
 
 
-def ncu_traffic(workload, tag="apply"):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one frame's launches of the phase `tag` ("apply": the update kernel(s), "solve3": the
-    persistent solve kernel of `fast`, "sort": the radix sort passes of `merged`), from the newest committed `ncu --set full` capture
-    (profiles/r*/prof_<tag>_<workload>*.raw.csv; one row per launch, summed) -> (bytes or None, which capture).  A capture describes the
-    kernels of the commit it was taken at; the directory carries the round."""
-    import csv
-    import glob
-    cands = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*", f"prof_{tag}_{workload}*.raw.csv")))
-    for path in reversed(cands):
-        try:
-            rows = [r for r in csv.reader(open(path)) if r]
-            hdr, units, launches = rows[0], rows[1], rows[2:]
-            scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-            tot = 0.0
-            for vals in launches:
-                for name in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    k = hdr.index(name)
-                    tot += float(vals[k].replace(",", "")) * scale.get(units[k], 1.0)
-            return tot, os.path.relpath(path, ROOT) + f" (ncu --set full, {len(launches)} launch(es) of one frame)"
-        except Exception:
-            continue
-    return None, None
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -228,7 +208,42 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
+
+
+def gpu_identity(gpu_index):
+    """Name and power limit of the card a number was measured on (they belong beside the number)."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={gpu_index}", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        name, limit = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit_w": float(limit)}
+    except Exception:
+        return None
+
+
+DUMP_BUDGET = 48 << 20   # bytes of sampled per-voxel arrays; the per-block arrays (40 B per block) come on top, 64 MB in all
+
+
+def dump_outputs(integ, out_dir):
+    """The map after the last timed step, as a caller of ksg_export_blocks receives it: blocks sorted by block index (the pool
+    order depends on allocation races), per-block index / observed-voxel count / weight sum of EVERY block, and every per-voxel
+    field of a fixed sample of blocks (seeded, sorted) small enough for DUMP_BUDGET.  uint8 fields become float32 (exact)."""
+    os.makedirs(out_dir, exist_ok=True)
+    exp = integ.export()
+    idx = exp["block_index"]
+    order = np.lexsort((idx[:, 2], idx[:, 1], idx[:, 0]))
+    nb = len(order)
+    per_block = sum(a[0].size for k, a in exp.items() if k != "block_index") * 4 if nb else 1
+    k = min(nb, DUMP_BUDGET // per_block)
+    pick = order[np.sort(np.random.default_rng(0).choice(nb, size=k, replace=False))] if k < nb else order
+    w = exp["tsdf_weight"][order].astype(np.float64)
+    arrays = {"block_index": idx[order].astype(np.float64), "block_observed_voxels": (w > 0).sum(axis=1).astype(np.float64),
+              "block_weight_sum": w.sum(axis=1), "sample_block_index": idx[pick].astype(np.float64)}
+    for name in ("tsdf_distance", "tsdf_weight", "tsdf_rgba", "sem_label", "sem_priors", "sem_rgba"):
+        arrays["sample_" + name] = exp[name][pick].astype(np.float32)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_reference(args):
@@ -320,8 +335,8 @@ def measure(args, workload, steps, warmup, ctx, with_cpu, profile_frames):
     n = warmup + steps
     spatial = args.sharding == "spatial" and world > 1
     # sequence mode (replicas): every rank integrates the SAME synthetic stream into its own map - weak scaling means fixed work per GPU
-    # (rank-specific trajectories differ by up to 10 % in voxel updates per frame, which the max over ranks then reports as lost efficiency:
-    # profiles/r02/bench_seq_fast5_n8.json, 18.4 K frames/s = 0.92 x 8 x the 1-GPU rate); KSG_BENCH_RANK_STREAMS=1 restores one trajectory per rank
+    # (rank-specific trajectories differ by up to 10 % in voxel updates per frame, which the max over ranks then reports as lost efficiency);
+    # KSG_BENCH_RANK_STREAMS=1 restores one trajectory per rank
     cam, frames = gen_frames(workload, n, rank if (not spatial and os.environ.get("KSG_BENCH_RANK_STREAMS")) else 0)
     P = w * h
 
@@ -367,7 +382,11 @@ def measure(args, workload, steps, warmup, ctx, with_cpu, profile_frames):
     prof = integ.get_profile()
     launches, libcalls = prof["kernel_launches"], prof["library_calls"]
     clocks = sampler.stop() if rank == 0 else None
+    if clocks is not None:
+        clocks["gpu"] = gpu_identity(local_rank)
     blocks = integ.num_blocks()
+    if args.dump_outputs and rank == 0 and workload == args.workload:
+        dump_outputs(integ, args.dump_outputs)
     if args.quick:
         integ.close()
         return {"workload": workload, "value": steps / (ms / 1e3), "ms_per_step": ms / steps, "quick": True,
@@ -523,8 +542,6 @@ def measure(args, workload, steps, warmup, ctx, with_cpu, profile_frames):
         if arm == "port":
             cpu["mvoxel_updates_per_s"] = c_all["mupdates_per_s"]
     head = e2e.get("pipelined", e2e["sync"])
-    tag_of_phase = ({"tile_apply": "apply"} if itype == KSG_INTEGRATOR_FAST else {"tile_apply": "apply", "record_sort": "sort"})
-    traffic, traffic_src = ncu_traffic(workload, tag_of_phase.get(top_phase, "solve3" if itype == KSG_INTEGRATOR_FAST else top_phase))
     shim = shim_e2e(workload, frames[warmup:], cam) if (world == 1 and args.shim_e2e) else None
     return {
         "metric": "depth_frames_per_s", "value": value, "unit": "frames/s", "n_gpus": world, "steps": steps,
@@ -535,8 +552,8 @@ def measure(args, workload, steps, warmup, ctx, with_cpu, profile_frames):
                                f"{'fast' if itype == KSG_INTEGRATOR_FAST else 'merged'} integrator (BASELINE.json configs)",
                    "name": workload, "voxels_per_side": 16, "frames_distinct": n, "merged_bundle_order": args.merged_bundle_order,
                    "hot_voxel_mode": int(args.hot_voxels),
-                   "l2_policy": f"every step reads a different frame ({total_in / 1e6:.0f} MB of inputs cycled, larger than the 126 MB L2 "
-                                "when steps >= 90) and a different part of the map; no explicit flush",
+                   "l2_policy": f"every step reads a different frame ({total_in / 1e6:.0f} MB of inputs cycled; the H100's L2 holds 50 MB) "
+                                "and a different part of the map; no explicit flush",
                    "parallelism": ("one map spatially sharded by tile owner over the GPUs; frames broadcast from rank 0 with NCCL" if spatial
                                    else "one sequence + map per GPU (the same synthetic stream on every rank), no collective") if world > 1 else "single GPU",
                    "map_blocks_after_run": blocks},
@@ -564,7 +581,7 @@ def measure(args, workload, steps, warmup, ctx, with_cpu, profile_frames):
                      "kernel": kernel_of_phase[top_phase], "phase": top_phase, "kernel_ms": top_ms,
                      "frame_frac": ach(frame_ms) / peak if peak else None, "frame_ms": frame_ms,
                      "tile_apply_frac": ach(apply_ms) / peak if peak and apply_ms > 0 else None, "tile_apply_ms": apply_ms,
-                     "traffic": traffic, "traffic_source": traffic_src, "peak_kind": peak_kind,
+                     "traffic": None, "traffic_source": "DRAM bytes are not measured by the benchmark (it runs no profiler)", "peak_kind": peak_kind,
                      "algorithmic_bytes_per_launch": alg_bytes,
                      "note": "algorithmic bytes of one frame = updates * (34 + 8 C) + pixels * 5 (SURVEY.md 8d); `frac` divides them by the duration of "
                              "the phase with the largest share of the frame (`kernel`), `frame_frac` by the whole frame, `tile_apply_frac` by the update "
@@ -671,6 +688,8 @@ def measure_frame_batches(args, workload, steps, warmup, ctx):
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms, wall_ms = float(t[0]), float(t[1])
     blocks = base.num_blocks()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(base, args.dump_outputs)    # rank 0's replica after the last timed batch
     base.close(); delta.close()
     if rank != 0:
         return None
@@ -714,6 +733,8 @@ def main():
     ap.add_argument("--sequences-per-gpu", type=int, default=4, help="N = 1, fast: also measure K independent sequences on one GPU (0/1: skip)")
     ap.add_argument("--quick", action="store_true", help="development aid: only the device-resident `value` leg, printed as a short line")
     ap.add_argument("--shim-e2e", type=int, default=1, help="N = 1: also time the C++ drop-in classes end to end (eager / lazy layer sync); 0 = skip")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the map of the timed integrator after its last step to DIR/<name>.npy (see dump_outputs)")
     ap.add_argument("--extra-workloads", default="merged2", help="comma list of further workloads measured (briefly) into `workloads` at N = 1; '' = none")
     args = ap.parse_args()
     if args.warmup < 3:

@@ -1,10 +1,10 @@
 /*
- * ksg.h — C-ABI of the B200-native semantic TSDF integrator ("ksg" = Kimera-Semantics on GPU).
+ * ksg.h — C-ABI of the H100-native semantic TSDF integrator ("ksg" = Kimera-Semantics on GPU).
  *
  * This header is the drop-in boundary. Everything above it (the C++ classes in
  * kimera_semantics_b200/cpp that mirror kimera::FastSemanticTsdfIntegrator /
  * kimera::MergedSemanticTsdfIntegrator / kimera::SemanticTsdfIntegratorFactory) is a thin
- * host shim; everything below it is hand-written sm_100a CUDA.  Signatures use plain
+ * host shim; everything below it is hand-written sm_90a CUDA.  Signatures use plain
  * pointers and sizes only (no torch / Eigen / voxblox types).
  *
  * Each entry point cites the reference interface it replaces (paths relative to the
@@ -363,7 +363,7 @@ int64_t ksg_debug_fast_timeline(ksg_integrator* h, int64_t* out80 /* 64 time mar
  * `merged` integrator (base.cpp:306-307).  Host buffers. */
 int32_t ksg_debug_chain_sum(const float* terms, int64_t n, float s0, float* result);
 
-/* Build information: "sm_100a" etc. */
+/* Build information: "sm_90a" etc. */
 const char* ksg_build_info(void);
 
 #ifdef __cplusplus

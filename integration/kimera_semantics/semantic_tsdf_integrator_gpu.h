@@ -1,5 +1,5 @@
 // semantic_tsdf_integrator_gpu.h -- the file a kimera_semantics maintainer adds next to semantic_tsdf_integrator_{fast,merged}.h
-// to route both integrator types to the B200 library (INTEGRATION.md section B).  It is written against the REFERENCE's headers
+// to route both integrator types to the H100 library (INTEGRATION.md section B).  It is written against the REFERENCE's headers
 // (kimera_semantics/semantic_integrator_base.h, voxblox/integrator/tsdf_integrator.h) and the C-ABI in include/ksg.h only; in this
 // repository it is compile- and link-checked against the reference's real kimera_semantics headers with `make -C oracle ref`
 // (oracle/_ref/gpu_binding_check; voxblox / Eigen / glog come from the stand-ins there, from the real packages in a catkin build).

@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI in include/ksg.h (the drop-in boundary).
 
-This is plumbing for tests and bench.py: it loads `csrc/libksg.so` (hand-written sm_100a CUDA behind
+This is plumbing for tests and bench.py: it loads `csrc/libksg.so` (hand-written sm_90a CUDA behind
 `extern "C"` entry points) and fails loudly when the library is missing — there is no CPU fallback.
 """
 from __future__ import annotations
@@ -142,7 +142,7 @@ def default_config(integrator_type: int = KSG_INTEGRATOR_FAST, voxel_size: float
     cfg.shard_rank = 0
     cfg.shard_count = 1
     cfg.merged_bundle_order = KSG_BUNDLE_ORDER_LIBSTDCXX   # the reference's order (merged.cpp:210-231)
-    cfg.hot_voxel_mode = 0   # opt-in: measured slower than the per-voxel kernels alone (profiles/r02/bench_merged2_hot.json)
+    cfg.hot_voxel_mode = 0   # opt-in: slower than the per-voxel kernels alone on merged2
     return cfg
 
 

@@ -1,5 +1,5 @@
 // Mirror of kimera_semantics/include/kimera_semantics/semantic_integrator_base.h (reference base.h:54-225) for the
-// B200 build: same ColorMode / SemanticConfig / constructor contract / public data members.  The per-voxel update
+// H100 build: same ColorMode / SemanticConfig / constructor contract / public data members.  The per-voxel update
 // (base.cpp:136-194) does not run on the host any more: it lives in the CUDA tile kernel behind include/ksg.h.
 #pragma once
 #include <memory>

@@ -1,5 +1,5 @@
 // Drop-in for kimera::FastSemanticTsdfIntegrator (reference fast.h:63-135): same base classes, constructor and
-// virtual integratePointCloud; the work is done by the sm_100a kernels behind include/ksg.h.
+// virtual integratePointCloud; the work is done by the sm_90a kernels behind include/ksg.h.
 #pragma once
 #include "kimera_semantics/gpu_integrator_core.h"
 namespace kimera {

@@ -1,6 +1,6 @@
 // ksg_api.cu — host side of the C-ABI in include/ksg.h: owns the device-resident map (spatial block hash +
 // tile pool), the per-frame scratch, and enqueues the kernel family of ksg_kernels.cuh.
-// Compiled for sm_100a only, with -fmad=false (bit-exact index arithmetic, see ksg_device.cuh).
+// Compiled for sm_90a (H100) only, with -fmad=false (bit-exact index arithmetic, see ksg_device.cuh).
 #include <cuda_runtime.h>
 #include <cub/cub.cuh>
 
@@ -51,7 +51,7 @@ struct ksg_integrator {
   ksg_config cfg{};
   DevCfg dc{};
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t own_stream = nullptr;
   std::string err;
   int deferred_status = 0;
@@ -169,7 +169,7 @@ struct ksg_integrator {
   int log_cap = 0;
   uint64_t* stamp64 = nullptr;       // [2][2^20] toggle stamps of solver 3
   int solve_smem = 0;
-  double clock_khz = 1965000.0;
+  double clock_khz = 1980000.0;
   // frames whose counters have not been read back yet (at most two: the counter copies land in two pinned slots)
   Counters* h_cnt_base = nullptr;    // [2] pinned; h_cnt points at the slot read last
   FastCounters* h_fc_base = nullptr; // [2] pinned
@@ -194,7 +194,7 @@ struct ksg_integrator {
   VoxelQueues vq{};
   cudaStream_t aux_stream = nullptr, aux_stream2 = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_join2 = nullptr;
-  // both measured SLOWER than what they were meant to replace (profiles/r02/bench_full_9.json vs bench_merged2_nohotk.json: the hot
+  // both were slower than what they were meant to replace when they were written (the hot
   // voxels' critical path is the TSDF weight recurrence, which a producer / consumer ring does not shorten; the warp-wide ray walk costs
   // more in rank searches than the scattered stores it saves) - kept as opt-in experiments: KSG_HOT_KERNEL=1, KSG_EMIT_WARP=1
   bool hot_kernel = false;
@@ -202,18 +202,18 @@ struct ksg_integrator {
   // shape of the two per-voxel kernels (environment: KSG_LONG_THREADS, KSG_LONG_GRID, KSG_SHORT_CTAS): the short-segment kernel is
   // capped at short_ctas CTAs per SM through a dynamic shared-memory reservation so that a CTA of the long-segment kernel (128
   // registers per thread) always finds room beside it - otherwise the two kernels run back to back
-  // (measured on merged2, profiles/r02/tuning_10.log: 6 CTAs/SM -> 148 fps, 4 + long 128 x 296 -> 163, 3 -> 166)
   int long_threads = 256, long_grid = 0, short_ctas = 3, short_smem = 0;
   bool short_thread = false;         // merged, C <= 32: k_voxel_apply_short_t
   // the non-hot long segments (0.3 ms standalone) run behind the short kernel on its stream instead of beside it (KSG_LONG_SERIAL=0:
-  // beside it): 202 against 199 frames/s with two short-kernel CTAs per SM (profiles/r02/tuning_18.log)
+  // beside it)
   bool long_serial = true;
-  int deep_threads = 128;            // block size of the hot-voxel instance (KSG_DEEP_THREADS): one warp per chain, 148 x 4 warps
+  int deep_threads = 128;            // block size of the hot-voxel instance (KSG_DEEP_THREADS): one warp per chain, 4 warps per CTA
   bool deep_hot = true;              // merged, C <= 32: the hot voxels go to the deep-pipeline instance of k_voxel_apply_long (KSG_DEEP_HOT=0: off)
-  // its CTAs per SM (KSG_SHORT_T_CTAS).  The frame is bound by the long-segment kernel (1184 warps, 128 registers each); whatever the
-  // short kernel takes from it costs more than it gains: merged2 1 -> 178 fps, 2 -> 166, 3 -> 166, 4 -> 170, warp-per-voxel kernel 170
-  // (profiles/r02/tuning_12.log)
-  int short_t_ctas = 2;              // (1 while the hot chains ran inside the long-segment kernel: tuning_12.log; 2 with the deep instance: tuning_18.log)
+  // its CTAs per SM (KSG_SHORT_T_CTAS).  The frame is bound by the long-segment kernel (128 registers per thread); whatever the
+  // short kernel takes from it costs more than it gains.  Re-measured on an H100 80GB HBM3 (400 W, merged2, bench.py --quick, two
+  // alternating passes): 1 -> 164 frames/s, 2 -> 181-182, 3 -> 171-173, 4 -> 177-178; KSG_LONG_THREADS=128 172-176,
+  // KSG_DEEP_THREADS=64 180-182, KSG_LONG_SERIAL=0 176-178 - the defaults below stay
+  int short_t_ctas = 2;
   int hot_smem = 0;
 
   long long* tile_debug = nullptr;  // optional per-tile (records, cycles) trace
@@ -1037,12 +1037,12 @@ void ksg_default_config(ksg_config* c, int32_t integrator_type, float voxel_size
   c->shard_rank = 0;
   c->shard_count = 1;
   c->merged_bundle_order = KSG_BUNDLE_ORDER_LIBSTDCXX;   // the reference's unordered_map iteration order (merged.cpp:210-231)
-  c->hot_voxel_mode = 0;   // opt-in (measured slower than the per-voxel kernels alone, profiles/r02/bench_merged2_hot.json)
+  c->hot_voxel_mode = 0;   // opt-in (slower than the per-voxel kernels alone on merged2)
 }
 
 #define KSG_STR_(x) #x
 #define KSG_STR(x) KSG_STR_(x)
-const char* ksg_build_info(void) { return "ksg abi " KSG_STR(KSG_ABI_VERSION) " sm_100a nvcc " KSG_STR(__CUDACC_VER_MAJOR__) "." KSG_STR(__CUDACC_VER_MINOR__) " built " __DATE__; }
+const char* ksg_build_info(void) { return "ksg abi " KSG_STR(KSG_ABI_VERSION) " sm_90a nvcc " KSG_STR(__CUDACC_VER_MAJOR__) "." KSG_STR(__CUDACC_VER_MINOR__) " built " __DATE__; }
 
 const char* ksg_last_error(const ksg_integrator* h) { return h ? h->err.c_str() : g_last_error.c_str(); }
 
@@ -1397,8 +1397,8 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     int coop = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, h->device);
     h->eval_grid = h->sm_count * std::max(1, std::min(per_sm, 4));
-    // measured on B200 (profiles/README.md): the persistent solver is ~3 % slower than launch-per-sweep (the sweeps, not the
-    // launches, dominate), so it is opt-in: KSG_PERSISTENT_EVAL=1
+    // the persistent solver is slower than launch-per-sweep (the sweeps, not the launches, dominate), so it is opt-in:
+    // KSG_PERSISTENT_EVAL=1
     h->persistent_eval = false;
     if (const char* e = std::getenv("KSG_PERSISTENT_EVAL")) h->persistent_eval = coop != 0 && per_sm > 0 && std::atoi(e) != 0;
   }

@@ -1,4 +1,4 @@
-// ksg_device.cuh — device-side arithmetic of the semantic TSDF integrator (sm_100a).
+// ksg_device.cuh — device-side arithmetic of the semantic TSDF integrator (sm_90a).
 //
 // Every float expression here is written in the operation order of the reference path so that
 // voxel / block indices come out bit-identical to the CPU integrator; the translation unit is

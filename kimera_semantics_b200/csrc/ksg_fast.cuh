@@ -25,7 +25,7 @@ namespace ksg {
 
 static constexpr int kCountBlock = 1024;      // pixels per block of k_fast_count / k_fast_classify (256 threads x 4)
 static constexpr int kEvalBlock = 512;        // sequence positions per block of k_fast_start_eval
-static constexpr int kSolveThreads = 1024;     // one CTA per SM: a grid barrier is 148 arrivals
+static constexpr int kSolveThreads = 1024;     // one CTA per SM: a grid barrier is one arrival per SM
 static constexpr int kFastKeyCap = 4096;      // update records of one tile sorted in shared memory (more: sorted in place in global memory)
 static constexpr int kFastPref = 1024;        // ... and whose per-record operands (point, label, colour) are prefetched into shared memory
 static constexpr int kTimelineSlots = 64;
@@ -54,8 +54,8 @@ struct VoxelUpdate { int bx, by, bz; uint32_t lin_label; float dist, wgt; uint32
 
 // observed-set solver, third formulation (ksg_fast3.cuh)
 // Rank groups (ranks [0, n) are final once converged, so the solver can finish a prefix of the rays before it starts the rest; the
-// following groups are group_mul x larger each).  Measured (profiles/r02/tuning_10.log, fast5): 512 -> 2047 fps, 2048 -> 2207, 8192 -> 2393,
-// one group for all rays -> 2494: every extra group costs more grid barriers than it saves work, so the default is ONE group
+// following groups are group_mul x larger each).  On fast5 every extra group cost more grid barriers than it saved work, so the
+// default is ONE group
 // (KSG_GROUP0 / KSG_GROUP_MUL keep the mechanism reachable).
 static constexpr int kGroup0 = 1 << 30;
 struct Cand;

@@ -1,6 +1,6 @@
 // ksg_fast3.cuh — observed-set solver, third formulation (round 2), used by k_fast_solve3.
 //
-// What the first measurements of the persistent kernel showed (profiles/r02/bench_fast5_v2.json: sweeps of 90 / 81 / 54 / 20 us):
+// What the first measurements of the persistent kernel showed (four sweeps, the first two the longest):
 //   * sweep 1 starts from "nothing but the guaranteed first steps is performed", so nearly every ray runs its full length
 //     (~1.9 M candidate steps materialised for ~57 K final updates), and sweep 2 takes almost all of it back;
 //   * every ray that toggles a slot re-evaluates itself in the next sweep (it sees its own stamp);
@@ -85,8 +85,8 @@ __device__ __forceinline__ int cand_insert3(const FastFrame& f, uint32_t slot, u
   return cand_insert_raw(f.o3.slot_cnt, f.o3.bkt, f.o3.head, f.o3.ovf, f.o3.ovf_cap, &f.fc->ovf_count, f.cnt, slot, entry);
 }
 
-// latest performed visit of `slot` that precedes `my_order`: its (value >> 20), or -1.  (A non-inlined variant of these helpers was measured
-// 20 % slower on the whole frame - profiles/r02/bench_full_9.json - so they stay inline; the loops past the first 8 entries are rolled.)
+// latest performed visit of `slot` that precedes `my_order`: its (value >> 20), or -1.  (A non-inlined variant of these helpers made the
+// whole frame slower, so they stay inline; the loops past the first 8 entries are rolled.)
 __device__ __forceinline__ int latest_performed_before_raw(const uint64_t* bkt, const int* slot_cnt, const int* head, const OvfEnt* ovf, int ovf_cap,
                                                         uint32_t slot, uint64_t my_order) {
   const ulonglong2* b = (const ulonglong2*)(bkt + (size_t)slot * kBkt3);

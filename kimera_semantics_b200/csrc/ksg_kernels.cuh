@@ -1,4 +1,4 @@
-// ksg_kernels.cuh — hand-written sm_100a kernels of the semantic TSDF integrator.
+// ksg_kernels.cuh — hand-written sm_90a kernels of the semantic TSDF integrator.
 //
 // Kernel family (SURVEY.md §7.4 numbering in brackets):
 //   k_depth_flags / k_classify      [K1]  back-projection, validity, dynamic-label filter, T_G_C * p

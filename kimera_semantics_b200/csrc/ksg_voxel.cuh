@@ -1,10 +1,8 @@
 // ksg_voxel.cuh — `merged`: per-VOXEL update kernels (round 2).
 //
 // Round 1 applied a frame's sorted update records with one CTA per touched 8^3 tile (k_tile_apply).  On the 2 cm workload
-// (31 M records, 4 690 tiles) that kernel ran 12.8 ms at 27 % SM-active: the tiles around the camera hold up to 1.1 M records each
-// and one CTA (8 warps) worked through such a tile alone while most SMs idled (profiles/r01/prof_apply_merged2.details.txt:
-// 2.28 G warp instructions = 1.9 ms of issue slots at full balance).  DRAM traffic was never the limit (0.7 %), so staging tiles in
-// shared memory bought nothing here.  This file drops the tile as the unit of work:
+// (31 M records, 4 690 tiles) the tiles around the camera hold up to 1.1 M records each, and one CTA (8 warps) worked through such
+// a tile alone while most SMs idled.  DRAM traffic was never the limit, so staging tiles in shared memory bought nothing here.  This file drops the tile as the unit of work:
 //
 //   k_voxel_heads        one thread per sorted record: detects voxel-segment heads, measures the segment (galloping search), and
 //                        files it by length: `long` (>= kLongLen records, one item per role) or `short`; tile heads do the updated()
@@ -601,9 +599,8 @@ __global__ void __launch_bounds__(256, 6) k_voxel_apply_short(DevCfg cfg, Xform 
 
 // ---------------------------------------------------------------------------------------------
 // short segments, C <= 32: one THREAD per voxel.
-// The warp-per-voxel kernel above spends ~900 warp instructions on a voxel that has ~11 records (ncu, profiles/r02/prof_apply_merged2:
-// 1.6 G warp instructions per frame, ALU pipe 63 % busy, 84 % of the SM's issue slots - compute bound on bookkeeping: the 32-lane weight
-// recurrence, the warp arg-max, per-voxel index arithmetic, a third of the lanes idle at C = 21).  Here a thread walks its voxel's records
+// The warp-per-voxel kernel above spends ~900 warp instructions on a voxel that has ~11 records (compute bound on bookkeeping: the
+// 32-lane weight recurrence, the warp arg-max, per-voxel index arithmetic, a third of the lanes idle at C = 21).  Here a thread walks its voxel's records
 // alone - the recurrences ARE sequential - and 32 voxels share every issued instruction.  Same operations in the same order per voxel as the
 // warp kernels (tsdf_measure + tsdf_chain_step per record, p[c] += row[c] in record order, first maximum wins), hence the same bits.
 // Rows of (L * freq) are read as 128-bit words from the zero-padded table tmp4.

@@ -2,8 +2,7 @@
 must hash to the digest of the reference's own sources - the one place where the default product deviates from the
 single-threaded reference (canonical first-insertion order, DESIGN.md section 4).
 
-The order algorithm is proven on the CPU against the real container in tests/test_unordered_map_order.py; on a B200 all 11
-`merged` cases came out bit-exact in every field (profiles/r01/merged_libstdcxx_bundle_order_gpu.log).  The check runs in a
+The order algorithm is proven on the CPU against the real container in tests/test_unordered_map_order.py.  The check runs in a
 subprocess (the mode is young: a device fault would stay contained instead of poisoning the CUDA context of the suite)."""
 import json
 import os

@@ -2,9 +2,8 @@
 tests/fuzz_cases.py (the oracle itself is held to the reference's own sources on the same cases in tests/test_oracle_vs_ref_fuzz.py).
 Block set, labels, colours, distances, weights and log-probabilities must all be bit-exact, and the per-frame counters equal.
 
-Status: the generator was written after round 1's GPU minutes were spent, so these cases (saturating max_weight, odd voxel sizes,
-points behind the camera, zero-weight points, random orientations, ...) first ran green on a B200 at the start of round 2 (profiles/r02/gpu_suite_start_of_round.log):
-XPASS once they do, and no effect on the rest of the suite (own process) if a corner case turns out to need work."""
+The cases cover saturating max_weight, odd voxel sizes, points behind the camera, zero-weight points, random orientations, ...;
+they run in their own process, so a corner case that needs work has no effect on the rest of the suite."""
 import json
 import os
 import subprocess

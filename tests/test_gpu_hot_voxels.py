@@ -3,8 +3,8 @@ tens of thousands of semantic updates per frame; their per-class float32 additio
 1024-record chunks by many warps instead of one warp's sequential loop.  The map must stay bit-identical to the oracle and the
 pre-pass must actually engage.
 
-Status: algorithm proven on the CPU (tools/exact_float_chain.py, csrc/test/chain_host_test.cpp); the kernels were written after round
-1's GPU minutes were spent; first green B200 run at the start of round 2 (own process).  The default path is provably untouched: the SASS
+Status: algorithm proven on the CPU (tools/exact_float_chain.py, csrc/test/chain_host_test.cpp); the GPU check runs in its own
+process.  The default path is provably untouched: the SASS
 of every existing k_tile_apply instantiation is identical up to one parameter offset."""
 import json
 import os

@@ -1,5 +1,5 @@
 // ubench_launch.cu — launch / barrier / graph overheads on the GPU box (decides how the `fast` frame is driven).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o ubench_launch ubench_launch.cu && ./ubench_launch
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o ubench_launch ubench_launch.cu && ./ubench_launch
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
