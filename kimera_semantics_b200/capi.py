@@ -487,7 +487,7 @@ class Integrator:
                 "phase0_us": {"file_shared_slot_visitors": us(0, 57) if t[57] else None, "sort_shared_slots": us(57, 58) if t[58] else None,
                               "scan_cast_counts": us(58 if t[58] else 0, 59), "compaction": us(59, 1)},
                 "debug": {"max_ray_setup_us": t[64] / (khz.value / 1e3), "max_ray_setup_insert_us": t[65] / (khz.value / 1e3),
-                          "max_ray_eval_us": t[67] / (khz.value / 1e3), "ray_evals": t[68], "blocks_evaluated": t[69], "blocks_materialised": t[70],
+                          "max_ray_eval_us": t[67] / (khz.value / 1e3), "ray_evals": t[68], "rays_scanned": t[66], "blocks_evaluated": t[69], "blocks_materialised": t[70],
                           "ray_evals_that_changed": t[71], "max_shared_slot_visitors": t[72], "shared_slot_visitors": t[73],
                           "shared_slots": t[74], "rays": t[75],
                           "max_setup_after_loads_us": t[76] / (khz.value / 1e3), "max_setup_after_init_us": t[77] / (khz.value / 1e3),

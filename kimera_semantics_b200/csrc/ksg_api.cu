@@ -155,12 +155,12 @@ struct ksg_integrator {
   int *tile_cnt = nullptr, *tile_slot = nullptr;
   TileDesc* tile_list = nullptr;
   int solve_grid = 0, apply_fast_smem = 0;
-  int solver = 3;                    // 3: rank-group solver (ksg_fast3.cuh), 2: first persistent formulation (k_fast_solve)
-  int solve_threads = kSolveThreads; // tuning knobs (environment): KSG_SOLVE_THREADS, KSG_SOLVE_CTAS_PER_SM, KSG_GROUP0, KSG_GROUP_MUL
-  int group0 = kGroup0, group_mul = 4;
+  int solver = 3;                    // 3: worklist solver (ksg_fast3.cuh), 2: first persistent formulation (k_fast_solve)
+  int solve_threads = kSolveThreads; // tuning knobs (environment): KSG_SOLVE_THREADS, KSG_SOLVE_CTAS_PER_SM
   Cand* cand16 = nullptr;
   OvfEnt* ovf = nullptr;
   RayRec* rayrec = nullptr;
+  int* wl = nullptr;                 // [3][max_points] solver 3: per-ray listed sweep, two scan lists
   int ovf_cap = 0;
   int *mixed_list = nullptr, *m_list = nullptr, *blk_run = nullptr;
   // update log (ksg_set_update_log): one entry per voxel the last frame updated
@@ -277,7 +277,7 @@ void free_all(ksg_integrator* h) {
                   h->ob.cand_next, h->ob.table, h->ks_sorted, h->seq_sorted, h->bstart, h->bundle_f, h->hist,
                   h->tmp, h->tmp4, h->b_key, h->b_base, h->bord_hash, h->bord_scratch, h->d_scan_tot, h->bundle_f2, h->d_hot_segs, h->d_hot_counts, h->d_hot_chunk_seg, h->d_hot_guess, h->d_hot_sums,
                   h->d_hot_tables, h->d_hot_prior, h->d_hot_same, h->tile_debug, h->d_gridbar, h->d_fc, h->blk_cnt, h->blk_off, h->warp_cnt, h->warp_off, h->seq_of_i, h->keys32,
-                  h->tile_cnt, h->tile_slot, h->tile_list, h->cand16, h->ovf, h->rayrec, h->mixed_list, h->m_list, h->blk_run, h->stamp64, h->d_log_head, h->d_log_prior, h->vq.long_items, h->vq.counters, h->rec_a, h->rec_b, h->tile_begin, h->cub_temp, h->d_in, h->d_exp, h->d_exp_slots};
+                  h->tile_cnt, h->tile_slot, h->tile_list, h->cand16, h->ovf, h->rayrec, h->wl, h->mixed_list, h->m_list, h->blk_run, h->stamp64, h->d_log_head, h->d_log_prior, h->vq.long_items, h->vq.counters, h->rec_a, h->rec_b, h->tile_begin, h->cub_temp, h->d_in, h->d_exp, h->d_exp_slots};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (h->h_cnt_base) cudaFreeHost(h->h_cnt_base);
   if (h->h_log_head) cudaFreeHost(h->h_log_head);
@@ -334,6 +334,7 @@ int reset_map(ksg_integrator* h, cudaStream_t s) {
     KSG_CUDA(cudaMemsetAsync(h->stamp64, 0x00, sizeof(uint64_t) * kSetSize, s));
     KSG_CUDA(cudaMemsetAsync(h->stamp64 + kSetSize, 0xFF, sizeof(uint64_t) * kSetSize, s));
   }
+  if (h->wl) KSG_CUDA(cudaMemsetAsync(h->wl, 0, sizeof(int) * (size_t)h->cap_points, s));   // listed sweeps: sweep ids restart at 0
   if (h->tile_cnt) KSG_CUDA(cudaMemsetAsync(h->tile_cnt, 0, sizeof(int) * (size_t)h->ht_cap * h->dc.tiles_per_block, s));
   h->n_pend = 0; h->n_stash = 0;
   std::memset(h->h_cnt_base, 0, 2 * sizeof(Counters));
@@ -531,8 +532,9 @@ int integrate_fast_v2(ksg_integrator* h, const InputDesc& in, const FrameIn& fin
   f.o3.cand = h->cand16; f.o3.ext_base = h->ob.ext_base; f.o3.cand_cap = h->ob.cand_cap; f.o3.slot_cnt = h->ob.slot_cnt; f.o3.bkt = h->ob.bkt;
   f.o3.head = h->ob.head; f.o3.ovf = h->ovf; f.o3.ovf_cap = h->ovf_cap; f.o3.stamp_max = h->stamp64; f.o3.stamp_min = h->stamp64 + kSetSize; f.o3.table = h->ob.table;
   f.rayrec = h->rayrec; f.blk_run = h->blk_run;
+  f.wl_listed = h->wl;
+  if (h->wl) { f.wl_list[0] = h->wl + h->cap_points; f.wl_list[1] = h->wl + 2 * (size_t)h->cap_points; }
   f.log_head = h->d_log_head; f.log_prior = h->d_log_prior; f.log_cap = h->log_cap;
-  f.group0 = h->group0; f.group_mul = h->group_mul;
   f.s_base = h->start_head; f.s_hmin = h->start_val; f.s_hmax = (uint32_t*)(h->clear_00 + (size_t)kSetSize * 5);
   f.s_visits = (int*)(h->clear_00 + (size_t)kSetSize * 9); f.mixed_list = h->mixed_list; f.m_list = h->m_list;
   const bool s3 = h->solver == 3;
@@ -1191,6 +1193,7 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
         h->ovf_cap = (int)std::min<long long>(std::max<long long>(1ll << 20, 4ll * (long long)N), 1ll << 28);
         KSG_CUDA(cudaMalloc((void**)&h->ovf, sizeof(OvfEnt) * (size_t)h->ovf_cap));
         KSG_CUDA(cudaMalloc((void**)&h->rayrec, sizeof(RayRec) * N));
+        KSG_CUDA(dmalloc(&h->wl, 3 * N));
         KSG_CUDA(dmalloc(&h->mixed_list, N)); KSG_CUDA(dmalloc(&h->m_list, N));
         KSG_CUDA(dmalloc(&h->blk_run, (size_t)(h->ob.cand_cap / 16 + 16)));
         KSG_CUDA(dmalloc(&h->stamp64, 2 * (size_t)kSetSize));
@@ -1369,8 +1372,6 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
       KSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fast_solve, kSolveThreads, 0));
       int per_sm3 = 0;
       if (const char* e = std::getenv("KSG_SOLVE_THREADS")) { const int t = std::atoi(e); if (t == 256 || t == 512 || t == 1024) h->solve_threads = t; }
-      if (const char* e = std::getenv("KSG_GROUP0")) h->group0 = std::max(32, std::atoi(e));
-      if (const char* e = std::getenv("KSG_GROUP_MUL")) h->group_mul = std::max(2, std::atoi(e));
       h->solve_smem = (int)(sizeof(int) * kSortPerWarp * (h->solve_threads / 32));
       KSG_CUDA(cudaFuncSetAttribute(k_fast_solve3, cudaFuncAttributeMaxDynamicSharedMemorySize, h->solve_smem));
       KSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm3, k_fast_solve3, h->solve_threads, (size_t)h->solve_smem));

@@ -43,6 +43,8 @@ struct FastCounters {      // device-resident state of the frame driver (persist
   int n_mixed;                               // start-set slots visited by more than one start cell this frame
   int m_cursor;                              // allocation cursor of their visitor lists
   int log_count;                             // update-log entries written by the frame (may exceed the capacity: then the log is incomplete)
+  int wl_claim[4];                           // solver 3, slot sweep & 3: next item of the sweep's scan list claimed by a warp
+  int wl_count[4];                           // ... rays on the sweep's scan list
   long long timeline[kTimelineSlots];        // clock64 of block 0 at the phase boundaries of k_fast_solve (profiling)
   long long dbg[16];                         // profiling only: maxima / counts gathered inside the solve kernel (see ksg_debug_fast_timeline)
 };
@@ -53,11 +55,6 @@ struct TileDesc { uint32_t tk; int n; long long off; };
 struct VoxelUpdate { int bx, by, bz; uint32_t lin_label; float dist, wgt; uint32_t rgba, srgba; };   // lin_label = linear voxel index | label << 24
 
 // observed-set solver, third formulation (ksg_fast3.cuh)
-// Rank groups (ranks [0, n) are final once converged, so the solver can finish a prefix of the rays before it starts the rest; the
-// following groups are group_mul x larger each).  On fast5 every extra group cost more grid barriers than it saved work, so the
-// default is ONE group
-// (KSG_GROUP0 / KSG_GROUP_MUL keep the mechanism reachable).
-static constexpr int kGroup0 = 1 << 30;
 struct Cand;
 struct OvfEnt;
 struct RayRec;
@@ -109,7 +106,8 @@ struct FastFrame {
   Obs3 o3;
   RayRec* rayrec;
   int* blk_run;              // consecutive-collision count at the start of every evaluation block (index: candidate index / 16)
-  int group0, group_mul;     // rank groups of the solver: first group, growth factor
+  int* wl_listed;            // per ray: the latest sweep whose scan list holds it (sweep ids are monotonic: never cleared per frame)
+  int* wl_list[2];           // scan lists of the sweeps after the second, slot sweep & 1
   // update log (NULL: off)
   VoxelUpdate* log_head; float* log_prior; int log_cap;
   // start set, third formulation: per-slot aggregates only (no linked lists)

@@ -6,10 +6,11 @@
 //   * every ray that toggles a slot re-evaluates itself in the next sweep (it sees its own stamp);
 //   * per candidate the solver chased four arrays (value, order, position, link).
 // Changes, none of which alters the fixpoint (DESIGN.md section 4: the dependency is triangular in rank order, the fixpoint unique):
-//   1. RANK GROUPS.  A ray depends only on rays of lower rank, so once ranks [0, n) have converged they are FINAL whatever the
-//      higher ranks do.  Rays are solved in groups of growing size (512, then x4); a group iterates to convergence against the
-//      finished lower groups.  With the `mixed` order the low ranks are a uniform sub-sample of the image, so a new group already
-//      sees most of the free space carved: its first evaluation is close to the answer, finished groups are never polled again.
+//   1. WORKLIST.  Sweeps 1 to 3 scan every ray; a later sweep k+1 scans only the rays evaluated in sweep k and the rays that
+//      examined a slot another ray toggled in sweep k (the slot's highest-ranked toggler of the sweep walks its bucket and
+//      overflow chain and lists them).  Every examined step is in its slot's bucket: performed steps as usual, the break step as
+//      a perf-0 entry.  Warps claim the rays of a sweep one at a time from a shared cursor, so a sweep ends with its last ray,
+//      not with the unluckiest warp.
 //   2. one 16-byte record per candidate {packed voxel index, bucket position, sweep of the owner's last toggle} and one per ray
 //      {materialised steps, updates, length, last evaluation}: one load each; the set value (hash + offset) is recomputed from the
 //      voxel index; flipping a candidate's "performed" bit is a plain store (the owner knows the whole entry).
@@ -19,6 +20,7 @@
 //      pass 1 commits the persistent table, allocates blocks and counts records per tile; pass 2 writes the (voxel, rank) keys
 //      straight into the tile's segment.  The voxel index kept per candidate replaces the second ray walk.
 #pragma once
+#include <cuda/atomic>
 #include "ksg_fast.cuh"
 
 namespace ksg {
@@ -65,8 +67,17 @@ __device__ __forceinline__ bool stamp_dirty(const Obs3& o, uint32_t slot, int la
 }
 
 // first time a candidate turns performed: it enters the slot's bucket (or the overflow pool); returns its position code.
-// The overflow push is one exchange, no retry loop and no fence: a reader that catches the entry half-written (pending link, fields of
-// an older frame) takes a wrong decision for this sweep only - the inserter stamps the slot afterwards, which marks that reader dirty.
+// The overflow push is one exchange, no retry loop.  The exchange releases the entry's fields and its pending link, and the link
+// is then stored with release: a reader that acquires the head and every link (ovf_next_acquire) sees every entry it reaches
+// complete, and the chain below it whole once the link resolves.  The chain walk of list_slot_visitors relies on that; the
+// collision readers of the same sweep need not wait, because the inserter stamps the slot, which marks them dirty.
+__device__ __forceinline__ int atom_exch_acq_rel(int* p, int v) {
+  return cuda::atomic_ref<int, cuda::thread_scope_device>(*p).exchange(v, cuda::memory_order_acq_rel);
+}
+__device__ __forceinline__ void st_release(int* p, int v) { cuda::atomic_ref<int, cuda::thread_scope_device>(*p).store(v, cuda::memory_order_release); }
+__device__ __forceinline__ int ld_acquire(const int* p) {
+  return cuda::atomic_ref<int, cuda::thread_scope_device>(*const_cast<int*>(p)).load(cuda::memory_order_acquire);
+}
 __device__ __forceinline__ int cand_insert_raw(int* slot_cnt, uint64_t* bkt, int* head, OvfEnt* ovf, int ovf_cap, int* ovf_count, Counters* cnt,
                                             uint32_t slot, uint64_t entry) {
   const int idx = atomicAdd(&slot_cnt[slot], 1);
@@ -77,8 +88,8 @@ __device__ __forceinline__ int cand_insert_raw(int* slot_cnt, uint64_t* bkt, int
   __stcg(&e->next, kOvfPending);
   __stcg(&e->order_perf, (entry & kEntPerf) | ((entry >> 13) & ((1ull << kEntOrderBits) - 1)));
   __stcg(&e->hi, (uint32_t)(entry & 0x1FFFull));
-  const int old = atomicExch(&head[slot], id);
-  __stcg(&e->next, old);
+  const int old = atom_exch_acq_rel(&head[slot], id);
+  st_release(&e->next, old);
   return -3 - id;
 }
 __device__ __forceinline__ int cand_insert3(const FastFrame& f, uint32_t slot, uint64_t entry) {
@@ -122,14 +133,22 @@ __device__ __forceinline__ int latest_performed_before3(const Obs3& o, uint32_t 
 }
 __device__ __forceinline__ bool later_performed_exists_raw(const uint64_t* bkt, const int* slot_cnt, const int* head, const OvfEnt* ovf, int ovf_cap,
                                                         uint32_t slot, uint64_t my_order) {
+  const ulonglong2* b = (const ulonglong2*)(bkt + (size_t)slot * kBkt3);
   const int total = __ldcg(&slot_cnt[slot]);
   const int n = total < kBkt3 ? total : kBkt3;
-  const uint64_t* b = bkt + (size_t)slot * kBkt3;
   bool later = false;
 #pragma unroll 1
-  for (int j = 0; j < n; ++j) {
-    const uint64_t e = __ldcg(&b[j]);
-    if ((e & kEntPerf) && ((e >> 13) & ((1ull << kEntOrderBits) - 1)) > my_order) later = true;
+  for (int q0 = 0; 2 * q0 < n && !later; q0 += 4) {       // 8 entries per round trip, as latest_performed_before_raw
+    ulonglong2 v[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) v[q] = __ldcg(b + q0 + q);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint64_t e2[2] = {v[q].x, v[q].y};
+#pragma unroll
+      for (int k = 0; k < 2; ++k)
+        if (2 * (q0 + q) + k < n && (e2[k] & kEntPerf) && ((e2[k] >> 13) & ((1ull << kEntOrderBits) - 1)) > my_order) later = true;
+    }
   }
   if (total > kBkt3) {
     int guard = total - kBkt3 + 8;
@@ -145,14 +164,65 @@ __device__ __forceinline__ bool later_performed_exists3(const Obs3& o, uint32_t 
   return later_performed_exists_raw(o.bkt, o.slot_cnt, o.head, o.ovf, o.ovf_cap, slot, my_order);
 }
 
+// ray r goes on the scan list of sweep `next`, at most once
+__device__ __forceinline__ void list_ray(const FastFrame& f, int r, int next) {
+  if (atomicMax(&f.wl_listed[r], next) < next) __stcg(&((next & 1) ? f.wl_list[1] : f.wl_list[0])[atomicAdd(&f.fc->wl_count[next & 3], 1)], r);
+}
+// Ray r toggled `slot` in sweep next-1 (>= 3): every other ray with an entry in the slot goes on the next scan list.  The rays that
+// need it were not evaluated in this sweep, so their entries date from earlier sweeps: their bucket words are visible after the
+// grid barrier, and their overflow entries lie below every entry pushed in this sweep.  A push of this sweep may be under way
+// while the walk runs; its link is acquired and waited for while it is still pending (cand_insert_raw), so the walk always
+// reaches the older part of the chain.  An entry written concurrently belongs to a ray evaluated in this sweep (listed anyway),
+// and a stale bucket word read in its place lists a ray for nothing (rank checked against n_cast).
+__device__ __forceinline__ int ovf_next_acquire(const FastFrame& f, int id) {
+  int nx = ld_acquire(&f.o3.ovf[id].next);
+  for (int spin = 0; nx == kOvfPending; ++spin) {   // the pusher stores the link right after its exchange
+    if (spin > (1 << 24)) { set_err(f.cnt, 2); return -1; }
+    nx = ld_acquire(&f.o3.ovf[id].next);
+  }
+  return nx;
+}
+__device__ __forceinline__ void list_slot_visitors(const FastFrame& f, uint32_t slot, int r, int next) {
+  const Obs3& o = f.o3;
+  const int n_cast = __ldcg(&f.cnt->n_cast);
+  const ulonglong2* b = (const ulonglong2*)(o.bkt + (size_t)slot * kBkt3);
+  const int total = __ldcg(&o.slot_cnt[slot]);
+  const int n = total < kBkt3 ? total : kBkt3;
+#pragma unroll 1
+  for (int q0 = 0; 2 * q0 < n; q0 += 2) {
+    ulonglong2 v[2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) v[q] = __ldcg(b + q0 + q);
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const uint64_t e2[2] = {v[q].x, v[q].y};
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int r2 = (int)(((e2[k] >> 13) & ((1ull << kEntOrderBits) - 1)) >> kOrderStepBits);
+        if (2 * (q0 + q) + k < n && r2 != r && r2 < n_cast) list_ray(f, r2, next);
+      }
+    }
+  }
+  if (total > kBkt3) {   // every entry reached was pushed this frame (the head starts at -1), so the chain ends at -1
+#pragma unroll 1
+    for (int id = ld_acquire(&o.head[slot]); id >= 0 && id < o.ovf_cap; id = ovf_next_acquire(f, id)) {
+      const int r2 = (int)((__ldcg(&o.ovf[id].order_perf) & ~kEntPerf) >> kOrderStepBits);
+      if (r2 != r && r2 < n_cast) list_ray(f, r2, next);
+    }
+  }
+}
+
 // single writer per candidate: the warp that owns the ray.  c.pos is updated when the candidate enters a bucket.
 // No fence between the entry and the stamp: a reader of the same sweep that misses the entry is flagged by the stamp (another
 // ray toggled its slot in its own sweep), and every store is visible after the grid barrier that ends the sweep.
-__device__ __forceinline__ void set_performed3(const FastFrame& f, Cand& c, long long ci, uint32_t slot, uint64_t order, uint64_t v, bool on, int sweep, int r) {
+// `enter` (with on = false): the ray's break step, examined but not performed, enters the bucket as a perf-0 entry so that a later
+// toggle of the slot finds the ray; it is stamped like a toggle because a reader may have caught the reserved entry unwritten.
+__device__ __forceinline__ void set_performed3(const FastFrame& f, Cand& c, long long ci, uint32_t slot, uint64_t order, uint64_t v, bool on,
+                                               bool enter, int sweep, int r) {
   const Obs3& o = f.o3;
   if (c.pos >= 0) __stcg(&o.bkt[c.pos], make_entry(on, order, v));
   else if (c.pos <= -3) __stcg(&o.ovf[-3 - c.pos].order_perf, (on ? kEntPerf : 0ull) | order);
-  else if (on) { c.pos = cand_insert3(f, slot, make_entry(true, order, v)); st_cand_state(&o.cand[ci], c.pos, 0); }
+  else if (on || enter) { c.pos = cand_insert3(f, slot, make_entry(on, order, v)); st_cand_state(&o.cand[ci], c.pos, 0); }
   else return;                       // never entered a bucket and stays unperformed: invisible to every other ray
   stamp_toggle(o, slot, sweep, r);
 }
@@ -167,7 +237,7 @@ __device__ __forceinline__ void set_performed3(const FastFrame& f, Cand& c, long
 // (else the caller walks serially: NaN / zero components follow the comparison semantics of the serial code).
 // ---------------------------------------------------------------------------------------------
 static constexpr int kWin = 64;               // steps per window (= the evaluation block)
-struct WarpDdaScratch { float a[3][kWin + 1]; int endc[4]; uint64_t out[kWin]; };
+struct WarpDdaScratch { float a[3][kWin + 1]; int endc[4]; uint64_t out[kWin]; int n_scanned; };   // n_scanned: profiling
 
 __device__ __forceinline__ bool ray_state_parallel_ok(const RayState& st) {
   const bool fin = isfinite(st.tn0) && isfinite(st.tn1) && isfinite(st.tn2) && isfinite(st.ts0) && isfinite(st.ts1) && isfinite(st.ts2);
@@ -274,17 +344,16 @@ __device__ __forceinline__ void fast3_ray_setup(const FastFrame& f, int r, int n
   if (f.profile) { dbg_max(f, 0, clock64() - t_begin); dbg_max(f, 1, t_ins); }
 }
 
-// One sweep over the rays [r_lo, r_hi): one warp per ray.  A ray is re-evaluated only from the first block that holds a dirty
-// step (the consecutive-collision count at every block start is kept), in blocks of up to 64 steps = two steps per lane; steps that
-// do not exist yet are produced by the warp-parallel ray walk.
-__device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r_lo, int r_hi, WarpDdaScratch* sc) {
+// Ray r in one sweep, by one warp.  A ray is re-evaluated only from the first block that holds a dirty step (the
+// consecutive-collision count at every block start is kept), in blocks of up to 64 steps = two steps per lane; steps that do not
+// exist yet are produced by the warp-parallel ray walk.  Returns (-1, -1) for a clean ray; for an evaluated one the steps it
+// toggled, [x, y] (empty when y < x, x >= 0).
+__device__ __forceinline__ int2 fast3_ray(const FastFrame& f, int r, int sweep, WarpDdaScratch* sc) {
   const Obs3& o = f.o3;
   const DevCfg& cfg = f.cfg;
   Counters* cnt = f.cnt;
   const int lane = threadIdx.x & 31;
-  const int warps_total = (gridDim.x * blockDim.x) >> 5;
-  if (blockIdx.x == 0 && threadIdx.x == 0) cnt->changed[(sweep + 1) & 3] = 0;
-  for (int r = r_lo + (threadIdx.x >> 5) * gridDim.x + blockIdx.x; r < r_hi; r += warps_total) {
+  {
     const int4 rr = __ldcg((const int4*)&f.rayrec[r]);
     int h = rr.x;
     const int old = rr.y, n = rr.z, last = rr.w;
@@ -299,7 +368,7 @@ __device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r
       }
       for (int d = 16; d > 0; d >>= 1) { const int t = __shfl_xor_sync(0xffffffffu, fd, d); fd = t < fd ? t : fd; }
     }
-    if (fd == 0x7fffffff) continue;
+    if (fd == 0x7fffffff) return make_int2(-1, -1);
     const long long t_eval = f.profile ? clock64() : 0;
     int n_blocks_eval = 0, n_blocks_mat = 0;
     int s0, blen;
@@ -310,6 +379,7 @@ __device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r
     while (s0 < n && U < 0) {
       const int cend = (s0 + blen < n) ? s0 + blen : n;
       ++n_blocks_eval;
+      bool fresh = false;   // the block's voxel keys are in sc->out, its candidates in no bucket
       if (s0 >= h) {   // materialise the block: continue the ray walk (A.7) from the saved state
         ++n_blocks_mat;
         int ok = 1;
@@ -331,6 +401,7 @@ __device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r
             else {
               for (int t = lane; t < W; t += 32) st_cand(&o.cand[base_ci + t], sc->out[t], -2, 0);
               if (lane == 0) f.ray_state[r] = st;
+              fresh = true;
             }
             __syncwarp();
           } else {
@@ -360,7 +431,11 @@ __device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r
       for (int q = 0; q < 2; ++q) {
         const int s = s0 + q * 32 + lane;
         c[q].vkey = 0; c[q].pos = -2; c[q].tog = 0; v[q] = 0; coll[q] = false;
-        if (s < cend) { c[q] = ld_cand(&o.cand[base_ci + q * 32 + lane]); v[q] = cand_value(c[q].vkey, f.set_offset); }
+        if (s < cend) {
+          if (fresh) c[q].vkey = sc->out[q * 32 + lane];
+          else c[q] = ld_cand(&o.cand[base_ci + q * 32 + lane]);
+          v[q] = cand_value(c[q].vkey, f.set_offset);
+        }
       }
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
@@ -382,10 +457,12 @@ __device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r
       }
       const int perf_end = (brk >= 0) ? brk : cend;
 #pragma unroll
-      for (int q = 0; q < 2; ++q) {                            // newly performed steps of this block
+      for (int q = 0; q < 2; ++q) {                            // newly performed steps of this block, the break step
         const int s = s0 + q * 32 + lane;
-        if (s < perf_end && s >= old)
-          set_performed3(f, c[q], base_ci + q * 32 + lane, (uint32_t)v[q] & kSetMask, ((uint64_t)r << kOrderStepBits) | (uint64_t)s, v[q], true, sweep, r);
+        const bool perf = s < perf_end && s >= old;
+        if (perf || (s == brk && c[q].pos == -2))
+          set_performed3(f, c[q], base_ci + q * 32 + lane, (uint32_t)v[q] & kSetMask, ((uint64_t)r << kOrderStepBits) | (uint64_t)s, v[q],
+                         perf, true, sweep, r);
       }
       __syncwarp();
       if (brk >= 0) { U = brk; break; }
@@ -398,7 +475,7 @@ __device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r
         const long long ci = cand_index3(o, f.ext_off, r, s);
         Cand c = ld_cand(&o.cand[ci]);
         const uint64_t v = cand_value(c.vkey, f.set_offset);
-        set_performed3(f, c, ci, (uint32_t)v & kSetMask, ((uint64_t)r << kOrderStepBits) | (uint64_t)s, v, false, sweep, r);
+        set_performed3(f, c, ci, (uint32_t)v & kSetMask, ((uint64_t)r << kOrderStepBits) | (uint64_t)s, v, false, false, sweep, r);
       }
     }
     if (lane == 0) {
@@ -406,19 +483,81 @@ __device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int r
       f.rayrec[r].eval_sweep = sweep;
       if (f.profile) { dbg_max(f, 3, clock64() - t_eval); dbg_add(f, 4, 1); dbg_add(f, 5, n_blocks_eval); dbg_add(f, 6, n_blocks_mat); if (U != old) dbg_add(f, 7, 1); }
     }
+    if (U != old) {   // every step this evaluation toggled lies in [lo, hi]
+      const int hi = U < old ? old : U;
+      return make_int2(U < old ? U : old, hi < h - 1 ? hi : h - 1);
+    }
   }
+  return make_int2(0, -1);
+}
+
+// After ray r's evaluation in sweep >= 3: lists the other visitors of every slot the evaluation toggled (steps [lo, hi]).  A slot
+// is walked when stamp_max (a max over sweep << 32 | rank) still names r, i.e. when r is the highest-ranked toggler of the slot
+// seen so far in this sweep; the highest-ranked toggler of the whole sweep therefore always walks it, after its own toggle.
+__device__ __forceinline__ void fast3_list_toggled(const FastFrame& f, int r, int sweep, int2 steps, int lane) {
+  const Obs3& o = f.o3;
+  const unsigned long long me = ((unsigned long long)(uint32_t)sweep << 32) | (uint32_t)r;
+  for (int s = steps.x + lane; s <= steps.y; s += 32) {
+    const Cand c = ld_cand(&o.cand[cand_index3(o, f.ext_off, r, s)]);
+    const uint32_t slot = (uint32_t)cand_value(c.vkey, f.set_offset) & kSetMask;
+    if (__ldcg((const unsigned long long*)&o.stamp_max[slot]) == me) list_slot_visitors(f, slot, r, sweep + 1);
+  }
+}
+
+// One sweep.  Sweeps 1 to 3 scan every ray in rank order (sweep 1 evaluates every ray); a later sweep scans the list the previous
+// sweep built.  Lists are built from sweep 3 on: sweep 2 takes back most of sweep 1's toggles, and listing them (the self-listing
+// of ~30 K evaluated rays on one counter, a bucket walk per toggled slot) cost more than the full scan of sweep 3 it saved.  The
+// first item of a warp is its warp index (consecutive items to different CTAs); the rest are claimed one at a time from a shared
+// cursor, so the sweep ends with its last ray.  (A claim is issued after the ray: one in flight during the evaluation would cost a
+// register, and spills.)
+// `it`: 1 for the frame's first sweep.
+__device__ __forceinline__ void fast3_sweep(const FastFrame& f, int sweep, int it, WarpDdaScratch* sc) {
+  const int lane = threadIdx.x & 31;
+  const bool all = it <= 3;
+  const bool track = it >= 3;
+  const int n_items = all ? __ldcg(&f.cnt->n_cast) : ((volatile int*)f.fc->wl_count)[sweep & 3];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {   // the counters of sweep+2 are idle until then: slot (sweep+2) & 3 was sweep-2's
+    f.cnt->changed[(sweep + 1) & 3] = 0;
+    f.fc->wl_claim[(sweep + 2) & 3] = 0;
+    f.fc->wl_count[(sweep + 2) & 3] = 0;
+  }
+  if (lane == 0) sc->n_scanned = 0;
+  __syncwarp();
+  const int warps_total = (gridDim.x * blockDim.x) >> 5;
+  int i = (threadIdx.x >> 5) * gridDim.x + blockIdx.x;
+  while (i < n_items) {
+    const int r = all ? i : __ldcg(&((sweep & 1) ? f.wl_list[1] : f.wl_list[0])[i]);   // (a select: an indexed parameter array goes to the stack)
+    const int2 toggled = fast3_ray(f, r, sweep, sc);
+    if (track && toggled.x >= 0) {   // evaluated: listed for the next sweep, and so are the other visitors of what it toggled
+      if (lane == 0) list_ray(f, r, sweep + 1);
+      fast3_list_toggled(f, r, sweep, toggled, lane);
+    }
+    if (f.profile && lane == 0) ++sc->n_scanned;
+    int next = 0;
+    if (lane == 0) next = warps_total + atomicAdd(&f.fc->wl_claim[sweep & 3], 1);
+    i = __shfl_sync(0xffffffffu, next, 0);
+  }
+  if (f.profile && lane == 0 && sc->n_scanned) dbg_add(f, 2, sc->n_scanned);   // rays scanned, one add per warp and sweep
 }
 
 // The performed candidates of every ray, 8 lanes per ray.  PASS 1: persistent table commit (the last performed visit of a slot
 // survives the frame), block allocation (base.cpp:205-254), records per tile.  PASS 2: (voxel, rank) key into the tile's segment.
+// The kernel's thread index (consecutive 32-item chunks on different CTAs), read afresh from the special registers: after the
+// sweeps it is recomputed, not carried (or spilled) through them.
+__device__ __forceinline__ int solve_gtid_fresh() {
+  unsigned t, b;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(b));
+  return (int)((((t >> 5) * gridDim.x + b) << 5) | (t & 31));
+}
+
 template <int PASS>
-__device__ __forceinline__ void fast3_walk_performed(const FastFrame& f, int n_cast, int n_tiles) {
+__device__ __forceinline__ void fast3_walk_performed(const FastFrame& f, int n_cast, int n_tiles, int gt) {
   constexpr int G = 8;
   const Obs3& o = f.o3;
   const DevCfg& cfg = f.cfg;
   const int groups_total = (gridDim.x * blockDim.x) / G;
   const int gl = threadIdx.x % G;
-  const int gt = ((((threadIdx.x >> 5) * gridDim.x + blockIdx.x) << 5) | (threadIdx.x & 31));   // CTA-balanced
   for (int r = gt / G; r < n_cast; r += groups_total) {
     const int U = __ldcg(&f.rayrec[r].L);
     for (int s = gl; s < U; s += G) {
@@ -453,7 +592,7 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
   unsigned int epoch = 0;
   unsigned int* bar = &f.fc->gridbar;
   const int lane = threadIdx.x & 31;
-  const int gtid = (((threadIdx.x >> 5) * gridDim.x + blockIdx.x) << 5) | lane;   // consecutive 32-item chunks go to different CTAs
+  const int gtid0 = (((threadIdx.x >> 5) * gridDim.x + blockIdx.x) << 5) | lane;   // consecutive 32-item chunks go to different CTAs
   const int gthreads = gridDim.x * blockDim.x;
   Counters* cnt = f.cnt;
   const int n_points = cnt->n_points;
@@ -463,7 +602,7 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
   // ---- phase 0a: start-set slots shared by several cells: every visitor files itself in the slot's list
   const int n_mixed = ((volatile int*)&f.fc->n_mixed)[0];
   if (n_mixed > 0) {
-    for (int seq = gtid; seq < n_points; seq += gthreads) {
+    for (int seq = gtid0; seq < n_points; seq += gthreads) {
       const uint64_t v = f.pt_key[seq];
       if (v == ~0ull) continue;
       const uint32_t slot = (uint32_t)v & kSetMask;
@@ -501,54 +640,49 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
   solve_barrier(bar, epoch);
   timeline_mark(f, 59);
   const int n_cast = ((volatile int*)&cnt->n_cast)[0];
-  for (int base = (gtid & ~31); base < n_points; base += gthreads) {
+  for (int base = (gtid0 & ~31); base < n_points; base += gthreads) {
     const int seq = base + lane;
     const bool c = seq < n_points && __ldcg(&f.cast_flag[seq]) != 0;
     const unsigned m = __ballot_sync(0xffffffffu, c);
     if (c) f.cast_seq[__ldcg(&f.warp_off[seq >> 5]) + __popc(m & ((1u << lane) - 1u))] = seq;
   }
   const int sweep_base0 = ((volatile int*)&f.fc->sweep_base)[0];   // sweep ids are monotonic across frames (31 bits: never wraps in practice)
-  const bool wrap = false;
+  if (gtid0 == 0) for (int k = 0; k < 4; ++k) { f.fc->wl_claim[k] = 0; f.fc->wl_count[k] = 0; }
   solve_barrier(bar, epoch);
   timeline_mark(f, tl++);
   // ---- phase 1: ray set-up (first kH0 steps of every ray)
-  for (int r0 = (gtid & ~31); r0 < n_cast; r0 += gthreads) fast3_ray_setup(f, r0 + lane, n_cast);
+  for (int r0 = (gtid0 & ~31); r0 < n_cast; r0 += gthreads) fast3_ray_setup(f, r0 + lane, n_cast);
   solve_barrier(bar, epoch);
   timeline_mark(f, tl++);
-  // ---- phase 2: observed-set fixpoint, rank group by rank group
-  int sweep = (wrap ? 0 : sweep_base0);
-  sweep = (sweep + 4) & ~3;       // counter slot (sweep + 1) & 3 of the first sweep was zeroed by the frame reset
-  const int first_sweep = sweep + 1;
-  bool failed = false;
-  int g_lo = 0, g_size = f.group0 > 0 ? f.group0 : kGroup0;
-  while (g_lo < n_cast && !failed) {
-    const int g_hi = (g_lo + g_size < n_cast) ? g_lo + g_size : n_cast;
-    bool converged = false;
-    for (int it = 0; it < max_sweeps; ++it) {
-      ++sweep;
-      fast3_sweep(f, sweep, g_lo, g_hi, (WarpDdaScratch*)(s_sort + (threadIdx.x >> 5) * kSortPerWarp));
-      solve_barrier(bar, epoch);
-      if (tl < kTimelineSlots - 12) timeline_mark(f, tl++);
-      const int changed = ((volatile int*)cnt->changed)[sweep & 3];
-      const int err = ((volatile int*)&cnt->err)[0];
-      if (err) { failed = true; break; }
-      if (!changed) { converged = true; break; }
-    }
-    if (!converged) failed = true;
-    g_lo = g_hi;
-    g_size = (g_size < (1 << 28)) ? g_size * (f.group_mul > 1 ? f.group_mul : 4) : g_size;
+  // ---- phase 2: observed-set fixpoint
+  // (n_cast and the frame's first sweep are not carried through the loop: registers there are the solver's)
+  int sweep = (sweep_base0 + 4) & ~3;   // counter slot (sweep + 1) & 3 of the first sweep was zeroed by the frame reset
+  bool converged = n_cast == 0;
+  int it = 0;
+  while (!converged && it < max_sweeps) {
+    ++it;
+    ++sweep;
+    fast3_sweep(f, sweep, it, (WarpDdaScratch*)(s_sort + (threadIdx.x >> 5) * kSortPerWarp));
+    solve_barrier(bar, epoch);
+    if (tl < kTimelineSlots - 12) timeline_mark(f, tl++);
+    const int changed = ((volatile int*)cnt->changed)[sweep & 3];
+    const int err = ((volatile int*)&cnt->err)[0];
+    if (err) break;
+    converged = !changed;
   }
+  const bool failed = !converged;
+  const int gtid = solve_gtid_fresh();
   if (gtid == 0) {
     cnt->last_sweep = sweep;
     f.fc->sweep_base = sweep;
-    f.fc->sweeps_last = sweep - first_sweep + 1;
+    f.fc->sweeps_last = it;
     if (failed && !((volatile int*)&cnt->err)[0]) set_err(cnt, 2 /*KSG_ERR_CUDA: the solver did not converge*/);
     if (f.profile) f.fc->timeline[kTimelineSlots - 1] = tl;
   }
   tl = kTimelineSlots - 12;
   timeline_mark(f, tl++);
   // ---- phase 3: table commit + block allocation + records per tile
-  if (!failed) fast3_walk_performed<1>(f, n_cast, 0);
+  if (!failed) fast3_walk_performed<1>(f, ((volatile int*)&cnt->n_cast)[0], 0, gtid);
   solve_barrier(bar, epoch);
   timeline_mark(f, tl++);
   timeline_mark(f, tl++);     // (slot kept for the layout of k_fast_solve: there the per-tile count is a phase of its own)
@@ -580,7 +714,7 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
   timeline_mark(f, tl++);
   // ---- phase 5: keys into the tile segments (the per-tile counters run back to zero: nothing to clear for the next frame)
   const bool ok2 = ((volatile int*)&cnt->err)[0] == 0 && !failed;
-  if (!failed) fast3_walk_performed<2>(f, n_cast, ok2 ? n_tiles : 0);
+  if (!failed) fast3_walk_performed<2>(f, ((volatile int*)&cnt->n_cast)[0], ok2 ? n_tiles : 0, gtid);
   if (gtid == 0) {
     int add = n_new;
     if (pool_base + add > f.map.max_blocks) add = f.map.max_blocks - pool_base;
@@ -591,7 +725,7 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
     f.fc->n_tile_list = 0;
     f.fc->rec_cursor = 0;
     f.fc->ovf_count = 0;
-    if (f.profile) { f.fc->dbg[10] = n_mixed; f.fc->dbg[11] = n_cast; }
+    if (f.profile) { f.fc->dbg[10] = ((volatile int*)&f.fc->n_mixed)[0]; f.fc->dbg[11] = ((volatile int*)&cnt->n_cast)[0]; }
     f.fc->n_mixed = 0;
     f.fc->m_cursor = 0;
     f.fc->log_count = 0;
