@@ -1,11 +1,13 @@
-// ksg_fast3.cuh — observed-set solver, third formulation (round 2), used by k_fast_solve3.
+// ksg_fast3.cuh — the `fast` integrator's observed-set solver, k_fast_solve3.
 //
-// What the first measurements of the persistent kernel showed (four sweeps, the first two the longest):
-//   * sweep 1 starts from "nothing but the guaranteed first steps is performed", so nearly every ray runs its full length
-//     (~1.9 M candidate steps materialised for ~57 K final updates), and sweep 2 takes almost all of it back;
-//   * every ray that toggles a slot re-evaluates itself in the next sweep (it sees its own stamp);
-//   * per candidate the solver chased four arrays (value, order, position, link).
-// Changes, none of which alters the fixpoint (DESIGN.md section 4: the dependency is triangular in rank order, the fixpoint unique):
+// voxel_observed_approx_set_ (fast.cpp:110-122, A.4) solved as a fixpoint:
+//   candidates  = ray steps materialised so far (the first kH0 of every cast ray, further steps of a ray once it is found to
+//                 survive that far),
+//   U[r]        = number of voxels ray r updates (= index of the step at which it breaks),
+//   a candidate (r,s) "collides" iff the latest PERFORMED candidate (s' < U[r']) that precedes it in (rank, step) order on the
+//   same slot carries the same value (none: the persistent table decides).
+// The dependency is triangular in rank order, so the fixpoint is unique (DESIGN.md section 4); sweeps re-evaluate rays until no
+// U changes, and in-place / asynchronous updates only accelerate convergence.  None of the following alters the fixpoint:
 //   1. WORKLIST.  Sweeps 1 to 3 scan every ray; a later sweep k+1 scans only the rays evaluated in sweep k and the rays that
 //      examined a slot another ray toggled in sweep k (the slot's highest-ranked toggler of the sweep walks its bucket and
 //      overflow chain and lists them).  Every examined step is in its slot's bucket: performed steps as usual, the break step as
@@ -14,11 +16,10 @@
 //   2. one 16-byte record per candidate {packed voxel index, bucket position, sweep of the owner's last toggle} and one per ray
 //      {materialised steps, updates, length, last evaluation}: one load each; the set value (hash + offset) is recomputed from the
 //      voxel index; flipping a candidate's "performed" bit is a plain store (the owner knows the whole entry).
-//   3. the per-slot stamp is (sweep << 8 | toggles in that sweep): a ray is NOT dirty when the only toggle of the slot in its last
-//      sweep was its own.
+//   3. per-slot toggle stamps (stamp_toggle): a ray is NOT dirty when the only toggle of the slot in its last sweep was its own.
 //   4. no record buffer: after convergence the performed candidates are walked twice, fully parallel (8 lanes per ray):
 //      pass 1 commits the persistent table, allocates blocks and counts records per tile; pass 2 writes the (voxel, rank) keys
-//      straight into the tile's segment.  The voxel index kept per candidate replaces the second ray walk.
+//      straight into the tile's segment.  The voxel index kept per candidate replaces a second ray walk.
 #pragma once
 #include <cuda/atomic>
 #include "ksg_fast.cuh"
@@ -96,8 +97,20 @@ __device__ __forceinline__ int cand_insert3(const FastFrame& f, uint32_t slot, u
   return cand_insert_raw(f.o3.slot_cnt, f.o3.bkt, f.o3.head, f.o3.ovf, f.o3.ovf_cap, &f.fc->ovf_count, f.cnt, slot, entry);
 }
 
+// two bucket entries of one 16-byte load: keeps the latest performed entry that precedes `my_order`
+__device__ __forceinline__ void scan_entries(const ulonglong2 v, int base, int n, uint64_t my_order, long long& best, int& best_hi) {
+  const uint64_t e2[2] = {v.x, v.y};
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const uint64_t e = e2[k];
+    const uint64_t eo = (e >> 13) & ((1ull << kEntOrderBits) - 1);
+    if (base + k < n && (e & kEntPerf) && eo < my_order && (long long)eo > best) { best = (long long)eo; best_hi = (int)(e & 0x1FFF); }
+  }
+}
 // latest performed visit of `slot` that precedes `my_order`: its (value >> 20), or -1.  (A non-inlined variant of these helpers made the
 // whole frame slower, so they stay inline; the loops past the first 8 entries are rolled.)
+// The slot's counter and the first 8 bucket entries are independent loads (one L2 round trip).  __ldcg: the structures change
+// while the sweep runs, L1 must not serve stale lines.
 __device__ __forceinline__ int latest_performed_before_raw(const uint64_t* bkt, const int* slot_cnt, const int* head, const OvfEnt* ovf, int ovf_cap,
                                                         uint32_t slot, uint64_t my_order) {
   const ulonglong2* b = (const ulonglong2*)(bkt + (size_t)slot * kBkt3);
@@ -685,7 +698,7 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
   if (!failed) fast3_walk_performed<1>(f, ((volatile int*)&cnt->n_cast)[0], 0, gtid);
   solve_barrier(bar, epoch);
   timeline_mark(f, tl++);
-  timeline_mark(f, tl++);     // (slot kept for the layout of k_fast_solve: there the per-tile count is a phase of its own)
+  timeline_mark(f, tl++);     // (an empty phase: the host reads the records -> tile segments span as marks tb+1 .. tb+4)
   const bool ok = ((volatile int*)&cnt->err)[0] == 0 && !failed;
   const int n_new_all = ((volatile int*)&cnt->n_new_blocks)[0];
   const int n_new = n_new_all < f.map.new_cap ? n_new_all : f.map.new_cap;
