@@ -553,7 +553,9 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   k_fast_start_eval3<<<(cap + kEvalBlock - 1) / kEvalBlock, kEvalBlock, 0, s>>>(f);
   if (h->profiling) cudaEventRecord(h->ev[1], s);
   {
-    int max_sweeps = 4096;   // theory: <= rays + 1 sweeps, practice 6-8; the kernel flags an error rather than spin for ever
+    // The fixpoint is reached within rays + 1 sweeps, plus one that changes nothing (DESIGN.md section 4), and a frame casts at
+    // most max_points rays: past this budget the solver is wrong, not slow, and the kernel flags an error rather than spin.
+    int max_sweeps = h->cap_points + 2;
     void* args[] = {(void*)&f, (void*)&max_sweeps};
     ++h->n_launches;
     KSG_CUDA(cudaLaunchCooperativeKernel((const void*)k_fast_solve3, dim3(h->solve_grid), dim3(h->solve_threads), args,

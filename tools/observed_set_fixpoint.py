@@ -92,6 +92,30 @@ def examined(vals: Sequence[int], u: int) -> range:
     return range(min(len(vals), u + 1))
 
 
+def slot_entries(rays, U) -> Dict[int, List[int]]:
+    """Per slot, the values of the entries the device's solution leaves in its bucket (and overflow chain): every performed
+    step and every breaking step, in (rank, step) order."""
+    out: Dict[int, List[int]] = {}
+    for vals, u in zip(rays, U):
+        for s in examined(vals, u):
+            out.setdefault(vals[s] & MASK, []).append(vals[s])
+    return out
+
+
+def table_collisions(rays, table, U) -> int:
+    """Collisions of the solution that the persistent table decides: steps whose slot no earlier examined step of the frame
+    visited, and whose value the table holds."""
+    seen = set()
+    n = 0
+    for vals, u in zip(rays, U):
+        for s in examined(vals, u):
+            k = vals[s] & MASK
+            if k not in seen and table.get(k) == vals[s]:
+                n += 1
+            seen.add(k)
+    return n
+
+
 def stamped_solve(rays, table, max_collisions, U_start, worklist: bool):
     """The device's iteration (ksg_fast3.cuh) on the Jacobi sweeps above.  A ray is re-evaluated only when it is DIRTY: never
     evaluated, or one of its examined slots was toggled (a step below U entered or left the performed set, or a breaking step
