@@ -363,6 +363,19 @@ int64_t ksg_debug_fast_timeline(ksg_integrator* h, int64_t* out80 /* 64 time mar
  * `merged` integrator (base.cpp:306-307).  Host buffers. */
 int32_t ksg_debug_chain_sum(const float* terms, int64_t n, float s0, float* result);
 
+/* Debug aid (not on the integration path): the TSDF recurrence of the warp-level apply kernels (tsdf_batch, csrc/ksg_kernels.cuh) on its
+ * own.  One warp walks the n records (sdf[k], uw[k], colour rgba_in[k] or (0,0,0,0) when NULL) in batches of 32, the last one partial,
+ * exactly as k_voxel_apply_long does, from the state (*dist, *wgt, *rgba), and writes the final state back; wide != 0 selects the
+ * instance of the deep-pipeline kernel.  Only default_truncation_distance and max_weight of cfg are read.  The result must equal n
+ * sequential updateTsdfVoxel state steps (tsdf_chain_step, csrc/ksg_device.cuh) bit for bit.  Host buffers. */
+int32_t ksg_debug_tsdf_batch(const ksg_config* cfg, int32_t wide, int64_t n, const float* sdf, const float* uw,
+                             const uint32_t* rgba_in /* or NULL */, int32_t keep_blend, float* dist, float* wgt, uint32_t* rgba);
+
+/* Debug aid (merged): how the LAST frame's voxels were routed by their record count.  out4[0]: voxels of the hot queue (>= 4096
+ * records), out4[1]: other long voxels, out4[2]: short voxels (all three 0 under the tile kernel, apply_mode 1), out4[3]:
+ * hot_voxel_mode 2, hot voxels whose TSDF recurrence was skipped because the frame provably leaves their saturated state as it is. */
+int32_t ksg_debug_apply_routes(ksg_integrator* h, int64_t* out4);
+
 /* Build information: "sm_90a" etc. */
 const char* ksg_build_info(void);
 

@@ -219,6 +219,11 @@ def load_library(path: Optional[str] = None):
     lib.ksg_integrate_depth_device_k64.restype = C.c_int32
     lib.ksg_debug_chain_sum.argtypes = [fp, C.c_int64, C.c_float, fp]
     lib.ksg_debug_chain_sum.restype = C.c_int32
+    u32p = C.POINTER(C.c_uint32)
+    lib.ksg_debug_tsdf_batch.argtypes = [C.POINTER(KsgConfig), C.c_int32, C.c_int64, fp, fp, u32p, C.c_int32, fp, fp, u32p]
+    lib.ksg_debug_tsdf_batch.restype = C.c_int32
+    lib.ksg_debug_apply_routes.argtypes = [H, C.POINTER(C.c_int64)]
+    lib.ksg_debug_apply_routes.restype = C.c_int32
     lib.ksg_unordered_map_schedule.argtypes = [C.c_int64, C.POINTER(C.c_int64)]
     lib.ksg_unordered_map_schedule.restype = C.c_int64
     lib.ksg_debug_fast_timeline.argtypes = [H, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_double)]
@@ -263,7 +268,7 @@ KSG_SYMBOLS = ["ksg_default_config", "ksg_create", "ksg_destroy", "ksg_last_erro
                "ksg_set_color_to_label", "ksg_sync", "ksg_num_blocks", "ksg_export_blocks", "ksg_export_blocks_by_index", "ksg_import_blocks",
                "ksg_last_updated_blocks", "ksg_reset", "ksg_build_info", "ksg_set_profiling", "ksg_get_profile", "ksg_debug_tile_times", "ksg_owner_mask",
                "ksg_unordered_map_schedule", "ksg_integrate_depth_k64", "ksg_integrate_depth_device_k64",
-               "ksg_debug_chain_sum", "ksg_debug_fast_timeline", "ksg_integrate_depth_async", "ksg_wait_frame",
+               "ksg_debug_chain_sum", "ksg_debug_tsdf_batch", "ksg_debug_apply_routes", "ksg_debug_fast_timeline", "ksg_integrate_depth_async", "ksg_wait_frame",
                "ksg_device_map_view", "ksg_merge_blocks_device", "ksg_copy_map_device", "ksg_integrate_image", "ksg_set_update_log", "ksg_fetch_update_log", "ksg_evaluate_labels", "ksg_extract_mesh", "ksg_clear_map", "ksg_copy_update_log_device", "ksg_merge_voxels_device"]
 
 
@@ -276,6 +281,22 @@ def debug_chain_sum(terms: np.ndarray, s0: float, lib=None) -> np.float32:
     if rc != 0:
         raise KsgError(f"ksg_debug_chain_sum failed: {KSG_STATUS.get(rc, rc)}")
     return out[0]
+
+
+def debug_tsdf_batch(cfg: KsgConfig, sdf, uw, dist, wgt, rgba=0, colors=None, keep_blend=False, wide=False, lib=None):
+    """One warp's tsdf_batch walk over the records (sdf[k], uw[k], colors[k]) from the state (dist, wgt, rgba); returns the final
+    (float32 dist, float32 wgt, uint32 rgba) (ksg_debug_tsdf_batch); needs a device."""
+    lib = lib or load_library()
+    s = np.ascontiguousarray(sdf, np.float32)
+    u = np.ascontiguousarray(uw, np.float32)
+    c = None if colors is None else np.ascontiguousarray(colors, np.uint32)
+    assert len(s) == len(u) and (c is None or len(c) == len(s))
+    d, w, r = C.c_float(float(dist)), C.c_float(float(wgt)), C.c_uint32(int(rgba))
+    rc = lib.ksg_debug_tsdf_batch(C.byref(cfg), int(wide), len(s), _ptr(s, C.c_float), _ptr(u, C.c_float), _ptr(c, C.c_uint32),
+                                  int(keep_blend), C.byref(d), C.byref(w), C.byref(r))
+    if rc != 0:
+        raise KsgError(f"ksg_debug_tsdf_batch failed: {KSG_STATUS.get(rc, rc)}")
+    return np.float32(d.value), np.float32(w.value), np.uint32(r.value)
 
 
 def unordered_map_schedule(n: int, lib=None) -> np.ndarray:
@@ -469,6 +490,12 @@ class Integrator:
         out["kernel_launches"] = int(launches.value)
         out["library_calls"] = int(libcalls.value)
         return out
+
+    def apply_routes(self) -> Dict[str, int]:
+        """merged: voxels of the last frame per apply route, and the hot voxels whose TSDF recurrence hot_voxel_mode 2 skipped."""
+        out = (C.c_int64 * 4)()
+        self._check(self.lib.ksg_debug_apply_routes(self.handle, out), "ksg_debug_apply_routes")
+        return {"hot": int(out[0]), "long": int(out[1]), "short": int(out[2]), "hot_tsdf_skipped": int(out[3])}
 
     def fast_timeline(self) -> Dict[str, object]:
         """Phase boundaries of the last frame's persistent solve kernel in microseconds from its start (fast integrator, profiling on)."""

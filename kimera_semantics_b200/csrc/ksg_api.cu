@@ -123,6 +123,8 @@ struct ksg_integrator {
   int* d_hot_same = nullptr;          // hot_voxel_mode 2
   long long hot_chunk_cap = 0;
   int64_t hot_segments_total = 0, hot_chunks_total = 0;
+  int last_hot_segments = 0;          // segments of the last frame's pre-pass (ksg_debug_apply_routes)
+  bool last_frame_queued = false;     // the last frame filled the per-voxel queues
 
   // records
   uint64_t *rec_a = nullptr, *rec_b = nullptr;
@@ -825,6 +827,8 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
   dev_err = h->h_cnt->err;
   h->num_blocks = h->h_cnt->pool_count;
   h->last_blocks_touched = h->h_cnt->n_blocks_touched;
+  h->last_hot_segments = (int)last_hot_voxels;
+  h->last_frame_queued = did_apply && h->voxel_apply;
   if (stats) {
     std::memset(stats, 0, sizeof(*stats));
     stats->points_in = h->h_cnt->n_points;
@@ -2079,6 +2083,81 @@ int32_t ksg_debug_chain_sum(const float* terms, int64_t n, float s0, float* resu
   if (d_terms) cudaFree(d_terms);
   if (d_out) cudaFree(d_out);
   return rc;
+}
+
+namespace {
+// one warp, the batch loop of k_voxel_apply_long's TSDF role with the measurements (sdf, uw, colour) given instead of computed
+__global__ void k_tsdf_batch_debug(TsdfParams tp, int wide, long long n, const float* __restrict__ sdf, const float* __restrict__ uw,
+                                   const uint32_t* __restrict__ col, int keep_blend, float* dist_io, float* wgt_io, uint32_t* rgba_io) {
+  const int lane = threadIdx.x & 31;
+  float dist = *dist_io, wgt = *wgt_io;
+  uint32_t rgba = *rgba_io;
+  __syncwarp();
+  for (long long base = 0; base < n; base += 32) {
+    const int nb = (n - base) < 32 ? (int)(n - base) : 32;
+    const float s = (lane < nb) ? sdf[base + lane] : 0.0f;
+    const float u = (lane < nb) ? uw[base + lane] : 0.0f;
+    const uint32_t c = (col && lane < nb) ? col[base + lane] : 0u;
+    if (wide) tsdf_batch<true>(tp, lane, nb, s, u, c, keep_blend != 0, dist, wgt, rgba);
+    else tsdf_batch<false>(tp, lane, nb, s, u, c, keep_blend != 0, dist, wgt, rgba);
+  }
+  if (lane == 0) { *dist_io = dist; *wgt_io = wgt; *rgba_io = rgba; }
+}
+}  // namespace
+
+int32_t ksg_debug_tsdf_batch(const ksg_config* cfg, int32_t wide, int64_t n, const float* sdf, const float* uw, const uint32_t* rgba_in,
+                             int32_t keep_blend, float* dist, float* wgt, uint32_t* rgba) {
+  if (!cfg || n < 0 || (n > 0 && (!sdf || !uw)) || !dist || !wgt || !rgba) return KSG_ERR_INVALID_ARGUMENT;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { cudaGetLastError(); return KSG_ERR_NO_DEVICE; }
+  TsdfParams tp{};
+  tp.voxel_size = cfg->voxel_size; tp.trunc = cfg->default_truncation_distance; tp.max_weight = cfg->max_weight;
+  tp.sparsity_factor = cfg->sparsity_compensation_factor;
+  tp.use_weight_dropoff = cfg->use_weight_dropoff; tp.use_sparsity = cfg->use_sparsity_compensation_factor;
+  // one buffer: [sdf n][uw n][colour n][dist, weight, rgba]
+  const size_t m = (size_t)std::max<int64_t>(n, 1);
+  uint32_t* d = nullptr;
+  int32_t rc = KSG_ERR_CUDA;
+  if (cudaMalloc((void**)&d, sizeof(uint32_t) * (3 * m + 3)) == cudaSuccess) {
+    float* d_sdf = (float*)d; float* d_uw = (float*)(d + m); uint32_t* d_col = d + 2 * m; uint32_t* d_state = d + 3 * m;
+    uint32_t state[3];
+    std::memcpy(&state[0], dist, 4); std::memcpy(&state[1], wgt, 4); state[2] = *rgba;
+    bool ok = cudaMemcpy(d_state, state, sizeof(state), cudaMemcpyHostToDevice) == cudaSuccess;
+    if (n > 0) {
+      ok = ok && cudaMemcpy(d_sdf, sdf, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess &&
+           cudaMemcpy(d_uw, uw, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess &&
+           (!rgba_in || cudaMemcpy(d_col, rgba_in, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess);
+    }
+    if (ok) {
+      k_tsdf_batch_debug<<<1, 32>>>(tp, wide, (long long)n, d_sdf, d_uw, rgba_in ? d_col : nullptr, keep_blend, (float*)d_state,
+                                    (float*)(d_state + 1), d_state + 2);
+      if (cudaMemcpy(state, d_state, sizeof(state), cudaMemcpyDeviceToHost) == cudaSuccess) {
+        std::memcpy(dist, &state[0], 4); std::memcpy(wgt, &state[1], 4); *rgba = state[2];
+        rc = KSG_OK;
+      }
+    }
+    cudaFree(d);
+  }
+  return rc;
+}
+
+int32_t ksg_debug_apply_routes(ksg_integrator* h, int64_t* out4) {
+  if (!h || !out4) return KSG_ERR_INVALID_ARGUMENT;
+  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
+  KSG_CUDA(cudaSetDevice(h->device));
+  KSG_CUDA(cudaDeviceSynchronize());
+  for (int i = 0; i < 4; ++i) out4[i] = 0;
+  if (h->last_frame_queued) {
+    int c[3] = {0, 0, 0};
+    KSG_CUDA(cudaMemcpy(c, h->vq.counters, sizeof(c), cudaMemcpyDeviceToHost));
+    out4[0] = c[0] / 2; out4[1] = c[1] / 2; out4[2] = c[2];   // a long voxel is two items, one per role
+  }
+  if (h->hot_enabled && h->cfg.hot_voxel_mode == 2 && h->last_hot_segments > 0) {
+    std::vector<int> same((size_t)h->last_hot_segments);
+    KSG_CUDA(cudaMemcpy(same.data(), h->d_hot_same, sizeof(int) * same.size(), cudaMemcpyDeviceToHost));
+    for (int v : same) out4[3] += v != 0;
+  }
+  return KSG_OK;
 }
 
 int64_t ksg_debug_tile_times(ksg_integrator* h, int32_t enable, int64_t capacity, int64_t* records_and_cycles) {

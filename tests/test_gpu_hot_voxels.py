@@ -5,7 +5,10 @@ pre-pass must actually engage.
 
 Status: algorithm proven on the CPU (tools/exact_float_chain.py, csrc/test/chain_host_test.cpp); the GPU check runs in its own
 process.  The default path is provably untouched: the SASS
-of every existing k_tile_apply instantiation is identical up to one parameter offset."""
+of every existing k_tile_apply instantiation is identical up to one parameter offset.
+
+The frames here never saturate a voxel (max_weight 10000), so mode 2 is checked for parity only; that its skip of a hot voxel at
+(+truncation, max_weight) is actually taken, and refused while the distance still moves, is asserted in test_gpu_apply_edges.py."""
 import json
 import os
 import subprocess
