@@ -262,11 +262,14 @@ int32_t ksg_merge_blocks_device(ksg_integrator* h, int64_t n_blocks, const void*
 int32_t ksg_copy_map_device(ksg_integrator* h, void* d_dst_pool, void* d_dst_keys, void* cuda_stream);
 
 /* Update log: the cheap way to keep HOST layers in step with the device map after every call (the reference's contract, base.cpp:257-265:
- * on return the caller reads the host Layer<> objects).  With a log of `capacity_voxels` entries switched on, every integrate call of the
- * `fast` integrator leaves one entry per voxel it updated (final distance, weight, colours, label and log-probabilities): kilobytes to a
- * few megabytes per frame instead of whole blocks.  ksg_fetch_update_log completes the last frame, copies its entries to page-locked host
- * memory owned by the library (two DMA transfers) and returns pointers that stay valid until the next call on this handle; *n = -1 and
- * KSG_ERR_SCRATCH_FULL when the frame updated more voxels than the log holds (use the block export then).  capacity 0 switches it off. */
+ * on return the caller reads the host Layer<> objects).  With a log of `capacity_voxels` entries switched on, every integrate call leaves
+ * one entry per voxel it updated (final distance, weight, colours, label and log-probabilities): a fraction of the bytes of the updated
+ * blocks.  Both integrators keep it: `fast` in its apply kernel (entries grouped by tile), `merged` in one extra pass behind its apply
+ * kernels (entries in (block index, tile, voxel) order, the same bytes on every run and whichever apply route ran; with spatial
+ * sharding, only the tiles this rank owns).  ksg_fetch_update_log completes the last frame, copies its entries to page-locked host memory owned by the library (two DMA
+ * transfers) and returns pointers that stay valid until the next call on this handle; *n = -1 and KSG_ERR_SCRATCH_FULL when the frame
+ * updated more voxels than the log holds (use the block export then; the map is complete either way).  capacity 0 switches it off;
+ * `merged` with the log off runs exactly the kernels it runs without one. */
 typedef struct ksg_voxel_update {
   int32_t block_index[3];
   uint32_t lin_label;       /* voxblox linear voxel index x + vps*(y + vps*z) in bits 0..23, semantic label in bits 24..31 */
@@ -277,7 +280,7 @@ int32_t ksg_set_update_log(ksg_integrator* h, int64_t capacity_voxels);
 int32_t ksg_fetch_update_log(ksg_integrator* h, int64_t* n, const ksg_voxel_update** updates, const float** sem_priors /* n * num_labels */);
 
 /* Voxel-granular deltas for the frame-per-GPU batch mode (DESIGN.md 8): the update log of a frame integrated into EMPTIED layers
- * (ksg_clear_map) lists exactly the voxels of that delta map with their final state.  ksg_copy_update_log_device copies the last frame's
+ * (ksg_clear_map) lists exactly the voxels of that delta map with their final state (either integrator).  ksg_copy_update_log_device copies the last frame's
  * log (n entries of ksg_voxel_update + n * num_labels floats) into caller-owned device buffers - the payload of an ncclAllGather; both
  * destinations NULL = size query.  ksg_merge_voxels_device merges n_deltas (<= 16) such logs, delta g at entry offset g * stride with
  * counts[g] valid entries (counts on the host), into this map in delta order with the arithmetic of ksg_merge_blocks_device: the two

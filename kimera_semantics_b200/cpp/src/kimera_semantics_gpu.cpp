@@ -177,10 +177,9 @@ GpuIntegratorCore::GpuIntegratorCore(int integrator_type, const vxb::TsdfIntegra
   if (const char* e = std::getenv("KSG_MERGED_BUNDLE_ORDER")) c.merged_bundle_order = std::atoi(e);
   const int rc = ksg_create(&c, &handle_);
   KSG_CHECK(rc == KSG_OK) << "ksg_create failed (" << rc << "): " << ksg_last_error(nullptr);
-  // eager layer sync of `fast` goes through the device-side update log (one entry per updated voxel); it must be on before the first frame
+  // eager layer sync goes through the device-side update log (one entry per updated voxel); it must be on before the first frame
   update_log_tried_ = true;
-  update_log_on_ = integrator_type == KSG_INTEGRATOR_FAST && std::getenv("KSG_NO_UPDATE_LOG") == nullptr &&
-                   ksg_set_update_log(handle_, 1 << 21) == KSG_OK;
+  update_log_on_ = std::getenv("KSG_NO_UPDATE_LOG") == nullptr && ksg_set_update_log(handle_, 1 << 21) == KSG_OK;
   // colour -> label table (color.cpp:69-82); alpha is forced to 255 by the callers
   std::vector<uint8_t> rgb, lab;
   for (const auto& kv : sc.semantic_label_to_color_->color_to_semantic_label_) {
@@ -207,9 +206,9 @@ void GpuIntegratorCore::integrate(const vxb::Transformation& T_G_C, const vxb::P
   if (sync_mode_ == LayerSyncMode::kEager) syncAfterCall();
 }
 
-// Eager sync (the reference's contract: the host layers hold the frame's result when integratePointCloud returns).  `fast` keeps an update
-// log on the device: one entry per updated voxel, fetched with two DMA transfers and written into the layers here; `merged` (and a frame
-// that overflows the log) copies the updated blocks.
+// Eager sync (the reference's contract: the host layers hold the frame's result when integratePointCloud returns).  Both integrators keep
+// an update log on the device: one entry per updated voxel, fetched with two DMA transfers and written into the layers here; a frame that
+// overflows the log (or KSG_NO_UPDATE_LOG) copies the updated blocks.
 void GpuIntegratorCore::syncAfterCall() {
   if (!update_log_on_) { syncUpdatedBlocks(); return; }
   int64_t n = 0;
@@ -224,7 +223,7 @@ void GpuIntegratorCore::syncAfterCall() {
   for (int64_t i = 0; i < n; ++i) {
     const ksg_voxel_update& u = up[i];
     const vxb::BlockIndex bi(u.block_index[0], u.block_index[1], u.block_index[2]);
-    if (!(bi == last_bi)) {           // entries come tile by tile: the block changes rarely
+    if (!(bi == last_bi)) {           // entries come tile by tile (`merged`: block by block): the block changes rarely
       last_bi = bi;
       tb = tsdf_layer_->allocateBlockPtrByIndex(bi);        // base.cpp:257-265: new blocks appear in both layers
       sb = semantic_layer_->allocateBlockPtrByIndex(bi);

@@ -21,6 +21,7 @@
 #include "ksg_fast.cuh"
 #include "ksg_fast3.cuh"
 #include "ksg_voxel.cuh"
+#include "ksg_log.cuh"
 #include "ksg_merge.cuh"
 #include "ksg_eval.cuh"
 #include "ksg_mesh.cuh"
@@ -162,6 +163,7 @@ struct ksg_integrator {
   VoxelUpdate *d_log_head = nullptr, *h_log_head = nullptr;
   float *d_log_prior = nullptr, *h_log_prior = nullptr;
   int log_cap = 0;
+  int64_t merged_log_count = 0;      // merged: entries of the last integrate call (ksg_merge_*_device reuse Counters, so it is kept here)
   int solve_smem = 0;
   double clock_khz = 1980000.0;
   // frames whose counters have not been read back yet (at most two: the counter copies land in two pinned slots)
@@ -329,6 +331,7 @@ int reset_map(ksg_integrator* h, cudaStream_t s) {
   h->frame_stamp = 0;
   h->last_blocks_touched = 0;
   h->deferred_status = 0;
+  h->merged_log_count = 0;
   KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
 }
@@ -614,6 +617,7 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
   if (cap == 0) {
     if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->blocks_allocated = h->num_blocks; }
     if (fast) { const int rcs = advance_sets(h, s); if (rcs) return rcs; }   // the sets are reset even for an empty frame
+    else h->merged_log_count = 0;
     h->last_blocks_touched = 0;
     return KSG_OK;
   }
@@ -634,6 +638,8 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
   if (fast) return integrate_fast(h, in, fin, T, cap, s, stats);
 
   // merged
+  h->merged_log_count = 0;
+  bool log_written = false;
   if (h->profiling) cudaEventRecord(h->ev[0], s);
   ++h->n_launches;
   k_frame_reset<<<1, 1, 0, s>>>(h->d_cnt, in.d_depth ? 0 : cap);
@@ -810,6 +816,35 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
     }
 #undef KSG_LAUNCH_APPLY
     }
+    if (h->d_log_head) {
+      // update log (ksg_log.cuh), behind every apply kernel.  The unsorted record buffer (and the short queue in it) is free again:
+      // [head record indices : n_records ints][flags : n_records bytes], later [head record indices][the same, block-index order].
+      // The sort keys go to the log's own entry buffer, which the entries overwrite only after the sort (32 bytes per entry >= 16).
+      int* heads = (int*)h->rec_a;
+      int* heads_alt = heads + n_records;
+      uint8_t* flags = (uint8_t*)heads_alt;
+      ++h->n_launches;
+      k_merged_log_heads<<<grid_for(n_records, B), B, 0, s>>>(dc, h->map, h->rec_b, n_records, flags);
+      size_t tb = h->cub_temp_bytes;
+      ++h->n_libcalls;
+      KSG_CUDA(cub::DeviceSelect::Flagged(h->cub_temp, tb, cub::CountingInputIterator<int>(0), flags, heads, &h->d_cnt->pad0, (int)n_records, s));
+      int n_heads = 0;
+      KSG_CUDA(cudaMemcpyAsync(&n_heads, &h->d_cnt->pad0, sizeof(int), cudaMemcpyDeviceToHost, s));
+      KSG_CUDA(cudaStreamSynchronize(s));
+      if (n_heads > 0 && n_heads <= h->log_cap) {
+        uint64_t* keys = (uint64_t*)h->d_log_head;
+        ++h->n_launches;
+        k_merged_log_keys<<<grid_for(n_heads, B), B, 0, s>>>(dc, h->map, h->rec_b, heads, n_heads, keys);
+        cub::DoubleBuffer<uint64_t> kb(keys, keys + n_heads);
+        cub::DoubleBuffer<int> vb(heads, heads_alt);
+        tb = h->cub_temp_bytes;
+        ++h->n_libcalls;
+        KSG_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_temp, tb, kb, vb, n_heads, 0, 63, s));   // pack_key: 3 x 21 bits
+        ++h->n_launches;
+        k_merged_log_write<<<h->sm_count * 8, 256, 0, s>>>(dc, h->map, h->rec_b, vb.Current(), n_heads, h->d_log_head, h->d_log_prior);
+      }
+      log_written = true;
+    }
   }
   if (h->profiling) { if (!did_apply) { cudaEventRecord(h->ev[4], s); cudaEventRecord(h->ev[5], s); } cudaEventRecord(h->ev[6], s); }
   ++h->n_launches;
@@ -828,6 +863,7 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
   h->num_blocks = h->h_cnt->pool_count;
   h->last_blocks_touched = h->h_cnt->n_blocks_touched;
   h->last_hot_segments = (int)last_hot_voxels;
+  if (log_written) h->merged_log_count = h->h_cnt->pad0;
   h->last_frame_queued = did_apply && h->voxel_apply;
   if (stats) {
     std::memset(stats, 0, sizeof(*stats));
@@ -1495,6 +1531,14 @@ int32_t ksg_wait_frame(ksg_integrator* h, ksg_frame_stats* stats) {
   return h->deferred_status ? h->fail(h->deferred_status, err_text(h->deferred_status)) : KSG_OK;
 }
 
+namespace {
+// entries of the last frame's update log: `fast` counts them in its frame counters, `merged` keeps the count of its last integrate call
+int64_t update_log_count(const ksg_integrator* h) {
+  if (h->cfg.integrator_type == KSG_INTEGRATOR_MERGED) return h->merged_log_count;
+  return h->h_fc ? h->h_fc->log_count : 0;
+}
+}  // namespace
+
 int32_t ksg_set_update_log(ksg_integrator* h, int64_t capacity_voxels) {
   if (!h || capacity_voxels < 0 || capacity_voxels > (1ll << 30)) return KSG_ERR_INVALID_ARGUMENT;
   auto fail = [&](int c, const char* m) { return h->fail(c, m); };
@@ -1506,9 +1550,25 @@ int32_t ksg_set_update_log(ksg_integrator* h, int64_t capacity_voxels) {
   if (h->h_log_head) cudaFreeHost(h->h_log_head);
   if (h->h_log_prior) cudaFreeHost(h->h_log_prior);
   h->d_log_head = nullptr; h->d_log_prior = nullptr; h->h_log_head = nullptr; h->h_log_prior = nullptr; h->log_cap = 0;
+  h->merged_log_count = 0;
   if (capacity_voxels == 0) return KSG_OK;
-  if (h->cfg.integrator_type != KSG_INTEGRATOR_FAST)
-    return fail(KSG_ERR_INVALID_ARGUMENT, "the update log is kept by the fast integrator's tile kernel only (merged: use ksg_export_blocks_by_index)");
+  if (h->cfg.integrator_type == KSG_INTEGRATOR_MERGED) {
+    // the merged log pass compacts the segment heads of up to rec_cap records in the unsorted record buffer (ksg_log.cuh)
+    if (h->rec_cap > 0x7fffffffll) return fail(KSG_ERR_INVALID_ARGUMENT, "update log: max_updates must be below 2^31 for the merged integrator");
+    size_t t = 0, t2 = 0;
+    KSG_CUDA(cub::DeviceSelect::Flagged(nullptr, t, cub::CountingInputIterator<int>(0), (uint8_t*)nullptr, (int*)nullptr, (int*)nullptr,
+                                        (int)h->rec_cap));
+    cub::DoubleBuffer<uint64_t> kb(nullptr, nullptr);
+    cub::DoubleBuffer<int> vb(nullptr, nullptr);
+    KSG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t2, kb, vb, (int)std::min<int64_t>(capacity_voxels, h->rec_cap), 0, 63));
+    t = std::max(t, t2);
+    if (t > h->cub_temp_bytes) {
+      if (h->cub_temp) cudaFree(h->cub_temp);
+      h->cub_temp = nullptr; h->cub_temp_bytes = 0;
+      KSG_CUDA(cudaMalloc(&h->cub_temp, t + 256));
+      h->cub_temp_bytes = t + 256;
+    }
+  }
   const size_t n = (size_t)capacity_voxels;
   KSG_CUDA(cudaMalloc((void**)&h->d_log_head, n * sizeof(VoxelUpdate)));
   KSG_CUDA(cudaMalloc((void**)&h->d_log_prior, n * sizeof(float) * h->dc.C));
@@ -1525,7 +1585,7 @@ int32_t ksg_fetch_update_log(ksg_integrator* h, int64_t* n_out, const ksg_voxel_
   if (!h->d_log_head) return fail(KSG_ERR_INVALID_ARGUMENT, "update log is off (ksg_set_update_log)");
   KSG_CUDA(cudaSetDevice(h->device));
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
-  const int64_t n = h->h_fc ? h->h_fc->log_count : 0;
+  const int64_t n = update_log_count(h);
   if (n > h->log_cap) { *n_out = -1; return fail(KSG_ERR_SCRATCH_FULL, "update log too small for this frame: fall back to ksg_last_updated_blocks / ksg_export_blocks_by_index"); }
   if (n > 0) {
     KSG_CUDA(cudaMemcpyAsync(h->h_log_head, h->d_log_head, (size_t)n * sizeof(VoxelUpdate), cudaMemcpyDeviceToHost, h->own_stream));
@@ -1929,7 +1989,7 @@ int32_t ksg_copy_update_log_device(ksg_integrator* h, int64_t* n_out, void* d_ds
   if (!h->d_log_head) return fail(KSG_ERR_INVALID_ARGUMENT, "update log is off (ksg_set_update_log)");
   KSG_CUDA(cudaSetDevice(h->device));
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
-  const int64_t n = h->h_fc ? h->h_fc->log_count : 0;
+  const int64_t n = update_log_count(h);
   if (n > h->log_cap) { *n_out = -1; return fail(KSG_ERR_SCRATCH_FULL, "update log too small for this frame"); }
   *n_out = n;
   if (!d_dst_updates && !d_dst_priors) return KSG_OK;                 // size query
