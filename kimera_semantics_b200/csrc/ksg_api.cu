@@ -217,6 +217,7 @@ struct ksg_integrator {
 
   // profiling
   bool profiling = false;
+  bool profile_marks_only = false;   // fast (KSG_PROFILE_MARKS_ONLY=1): the solve kernel's phase marks without its per-ray probes
   cudaEvent_t ev[KSG_NUM_PHASES + 1] = {};
   double phase_ms[KSG_NUM_PHASES] = {};
   int64_t prof_frames = 0;
@@ -513,7 +514,8 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   f.n_count_blocks = (cap + kCountBlock - 1) / kCountBlock;
   f.vec_ok = in.d_depth ? (((uintptr_t)in.d_depth % 16 == 0 && (uintptr_t)in.d_label_img % 4 == 0) ? 1 : 0) : 0;
   f.frame_stamp = h->frame_stamp;
-  f.profile = h->profiling ? 1 : 0;
+  f.profile = (h->profiling && !h->profile_marks_only) ? 1 : 0;
+  f.prof_marks = h->profiling ? 1 : 0;
   f.seq_of_i = sorted ? h->seq_of_i : nullptr;
   f.block_cnt = h->blk_cnt; f.block_off = h->blk_off; f.warp_cnt = h->warp_cnt; f.warp_off = h->warp_off;
   f.pt_pG = h->pt_pG; f.pt_label = h->pt_label; f.pt_flags = h->pt_flags; f.pt_color = h->pt_color; f.pt_key = h->pt_key;
@@ -1286,6 +1288,7 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
                                                                 "(k_fast_solve3 needs a cooperative launch with at least one CTA per SM)");
       h->solve_grid = h->sm_count * std::max(1, per_sm);
       if (const char* e = std::getenv("KSG_SOLVE_CTAS_PER_SM")) h->solve_grid = h->sm_count * std::max(1, std::min(per_sm, std::atoi(e)));
+      if (const char* e = std::getenv("KSG_PROFILE_MARKS_ONLY")) h->profile_marks_only = std::atoi(e) != 0;
       int khz = 0;
       if (cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, h->device) == cudaSuccess && khz > 0) h->clock_khz = khz;
     }

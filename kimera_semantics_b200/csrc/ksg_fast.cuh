@@ -90,7 +90,9 @@ struct FastFrame {
   int n_count_blocks;        // blocks of k_fast_count / k_fast_classify (depth entry)
   int vec_ok;                // depth / label pointers allow 128-bit / 32-bit vector loads
   int frame_stamp;
-  int profile;
+  int profile;               // per-ray / per-slot probes of the solve kernel (FastCounters::dbg): same-address atomics that slow the
+                             // phases they probe, the ray set-up the most
+  int prof_marks;            // block 0 of the solve kernel stamps clock64 at every phase boundary (FastCounters::timeline)
   const int* seq_of_i;       // "sorted" order mode: sequence position of input index i, else NULL (mixed: closed form)
   int* block_cnt; int* block_off;     // finite pixels per 1024-pixel block
   int* warp_cnt; int* warp_off;       // cast points per 32 sequence positions
@@ -420,7 +422,7 @@ __device__ __forceinline__ void solve_barrier(unsigned int* bar, unsigned int& e
 __device__ __forceinline__ void dbg_max(const FastFrame& f, int k, long long v) { if (f.profile) atomicMax((unsigned long long*)&f.fc->dbg[k], (unsigned long long)v); }
 __device__ __forceinline__ void dbg_add(const FastFrame& f, int k, long long v) { if (f.profile) atomicAdd((unsigned long long*)&f.fc->dbg[k], (unsigned long long)v); }
 __device__ __forceinline__ void timeline_mark(const FastFrame& f, int slot) {
-  if (f.profile && blockIdx.x == 0 && threadIdx.x == 0 && slot < kTimelineSlots) f.fc->timeline[slot] = clock64();
+  if (f.prof_marks && blockIdx.x == 0 && threadIdx.x == 0 && slot < kTimelineSlots) f.fc->timeline[slot] = clock64();
 }
 
 // SemanticVoxel / TsdfVoxel default construction of the frame's new blocks (semantic_voxel.h:14-27), all CTAs
