@@ -319,6 +319,37 @@ int32_t ksg_extract_mesh(ksg_integrator* h, float min_weight, int64_t vertex_cap
                          uint8_t* rgba /* 4 per vertex */, uint8_t* labels /* 1 per vertex */, int64_t block_capacity,
                          int32_t* block_index /* 3 per block */, int64_t* block_first_vertex, int64_t* n_vertices, int64_t* n_blocks);
 
+/* Point queries on the device map: what a host caller asks voxblox through Layer::getVoxelPtrByCoordinates and Interpolator<TsdfVoxel>
+ * (getDistance / getGradient with interpolate = true), without copying the map out.  Restates voxblox (not under the reference tree:
+ * unpinned; csrc/ksg_query.cuh lists the conventions).  Per point p (xyz_G: 3 floats, world frame):
+ *   - the containing voxel g = floor(p / voxel_size + 1e-6) (the integrator's own index arithmetic): KSG_QUERY_ALLOCATED when its block
+ *     is in the map, KSG_QUERY_OBSERVED when also weight > min_weight (the mesher's rule, voxblox default 1e-4).  tsdf_* and sem_* hold
+ *     that voxel (the fields and row layout of ksg_export_blocks) whenever ALLOCATED is set, also for an unobserved voxel;
+ *   - distance: the trilinear TSDF distance over the 8 voxel centres around p, KSG_QUERY_INTERPOLATED when all 8 are allocated and observed;
+ *   - gradient: central differences (D(p + vs e_a) - D(p - vs e_a)) / (2 vs) of that distance, KSG_QUERY_GRADIENT when all six are valid.
+ * What is not valid is NaN for floats and 0 for bytes; a non-finite point, or one outside the index range, has flags 0.  Every pointer of
+ * ksg_query_out may be NULL (= not wanted) and an unwanted array is never written.  Rejected (KSG_ERR_INVALID_ARGUMENT): n < 0, a NaN or
+ * negative min_weight, n > 0 with a NULL xyz_G, a NULL out, and a spatially sharded integrator (shard_count > 1: a rank holds only the
+ * tiles it owns).  n = 0, or no output wanted, returns KSG_OK without touching the device (the host entry still completes the pending
+ * frame).
+ * ksg_query_points: host buffers; completes the pending frame first (like ksg_extract_mesh), then stages, runs and returns when done.
+ * ksg_query_points_device: xyz_G and the arrays of *out are DEVICE memory (the struct itself is read on the host during the call); the call
+ * only enqueues the query on `cuda_stream` (NULL = the integrator's own stream, the one the host-buffer entries use) and sees every frame
+ * enqueued before it on that same stream, including merged's apply kernels on its side streams (the frame joins them back).  Ordering
+ * against work on other streams is the caller's job, as is keeping the outputs alive until the stream reaches them; as for every entry,
+ * calls on one handle must not overlap. */
+enum { KSG_QUERY_ALLOCATED = 1, KSG_QUERY_OBSERVED = 2, KSG_QUERY_INTERPOLATED = 4, KSG_QUERY_GRADIENT = 8 };
+typedef struct ksg_query_out {
+  uint8_t* flags;                                                  /* n   KSG_QUERY_* */
+  float* tsdf_distance; float* tsdf_weight; uint8_t* tsdf_rgba;     /* n, n, 4n   containing voxel */
+  uint8_t* sem_label; float* sem_priors; uint8_t* sem_rgba;         /* n, n*C, 4n containing voxel */
+  float* distance;                                                 /* n   trilinear TSDF distance */
+  float* gradient;                                                 /* 3n  central differences of the trilinear distance */
+} ksg_query_out;
+int32_t ksg_query_points(ksg_integrator* h, int64_t n, const float* xyz_G, float min_weight, const ksg_query_out* out);
+int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, float min_weight, const ksg_query_out* d_out,
+                                void* cuda_stream);
+
 /* Remove every block but keep the integrator: what Layer::removeAllBlocks() on both layers does to a live reference integrator.  The
  * fast integrator's two per-scan approximate sets (members of the integrator, fast.h:114-130) keep their contents and offsets, so the
  * next frame is integrated exactly as the reference integrator object would integrate it into its emptied layers.  Used by the

@@ -90,6 +90,18 @@ class KsgFrameStats(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
 
 
+KSG_QUERY_ALLOCATED = 1
+KSG_QUERY_OBSERVED = 2
+KSG_QUERY_INTERPOLATED = 4
+KSG_QUERY_GRADIENT = 8
+QUERY_FIELDS = ("flags", "tsdf_distance", "tsdf_weight", "tsdf_rgba", "sem_label", "sem_priors", "sem_rgba", "distance", "gradient")
+
+
+class KsgQueryOut(C.Structure):
+    """Mirror of `struct ksg_query_out` (include/ksg.h): one pointer per output, NULL = not wanted."""
+    _fields_ = [(name, C.c_void_p) for name in QUERY_FIELDS]
+
+
 def label_palette(num_labels: int) -> np.ndarray:
     """A deterministic label -> RGBA table (label 0 = white as color.cpp:64-66 forces)."""
     pal = np.zeros((256, 4), dtype=np.uint8)
@@ -254,6 +266,10 @@ def load_library(path: Optional[str] = None):
     lib.ksg_copy_update_log_device.restype = C.c_int32
     lib.ksg_merge_voxels_device.argtypes = [H, C.c_int32, C.POINTER(C.c_int64), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.ksg_merge_voxels_device.restype = C.c_int32
+    lib.ksg_query_points.argtypes = [H, C.c_int64, C.c_void_p, C.c_float, C.POINTER(KsgQueryOut)]
+    lib.ksg_query_points.restype = C.c_int32
+    lib.ksg_query_points_device.argtypes = [H, C.c_int64, C.c_void_p, C.c_float, C.POINTER(KsgQueryOut), C.c_void_p]
+    lib.ksg_query_points_device.restype = C.c_int32
     lib.ksg_clear_map.argtypes = [H]
     lib.ksg_clear_map.restype = C.c_int32
     lib.ksg_build_info.argtypes = []
@@ -269,7 +285,8 @@ KSG_SYMBOLS = ["ksg_default_config", "ksg_create", "ksg_destroy", "ksg_last_erro
                "ksg_last_updated_blocks", "ksg_reset", "ksg_build_info", "ksg_set_profiling", "ksg_get_profile", "ksg_debug_tile_times", "ksg_owner_mask",
                "ksg_unordered_map_schedule", "ksg_integrate_depth_k64", "ksg_integrate_depth_device_k64",
                "ksg_debug_chain_sum", "ksg_debug_tsdf_batch", "ksg_debug_apply_routes", "ksg_debug_fast_timeline", "ksg_integrate_depth_async", "ksg_wait_frame",
-               "ksg_device_map_view", "ksg_merge_blocks_device", "ksg_copy_map_device", "ksg_integrate_image", "ksg_set_update_log", "ksg_fetch_update_log", "ksg_evaluate_labels", "ksg_extract_mesh", "ksg_clear_map", "ksg_copy_update_log_device", "ksg_merge_voxels_device"]
+               "ksg_device_map_view", "ksg_merge_blocks_device", "ksg_copy_map_device", "ksg_integrate_image", "ksg_set_update_log", "ksg_fetch_update_log", "ksg_evaluate_labels", "ksg_extract_mesh", "ksg_clear_map", "ksg_copy_update_log_device", "ksg_merge_voxels_device",
+               "ksg_query_points", "ksg_query_points_device"]
 
 
 def debug_chain_sum(terms: np.ndarray, s0: float, lib=None) -> np.float32:
@@ -613,6 +630,28 @@ class Integrator:
                                               lab.ctypes.data_as(C.c_void_p), b, bidx.ctypes.data_as(C.c_void_p), first.ctypes.data_as(C.c_void_p),
                                               C.byref(nv), C.byref(nb)), "ksg_extract_mesh")
         return {"vertices": vtx, "rgba": rgba, "labels": lab, "block_index": bidx, "block_first": first}
+
+    def query_points(self, xyz, min_weight: float = 1e-4, priors: bool = True) -> Dict[str, np.ndarray]:
+        """Point queries on the device map (ksg_query_points): dict(flags [n] u8 (KSG_QUERY_*), tsdf_distance / tsdf_weight [n] f32,
+        tsdf_rgba [n, 4] u8, sem_label [n] u8, sem_priors [n, C] f32 (only with priors=True), sem_rgba [n, 4] u8 of the containing voxel,
+        distance [n] f32 trilinear, gradient [n, 3] f32).  Invalid entries are NaN / 0, see include/ksg.h."""
+        p = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+        n, nl = len(p), self.cfg.num_labels
+        out = {"flags": np.zeros(n, np.uint8), "tsdf_distance": np.zeros(n, np.float32), "tsdf_weight": np.zeros(n, np.float32),
+               "tsdf_rgba": np.zeros((n, 4), np.uint8), "sem_label": np.zeros(n, np.uint8), "sem_rgba": np.zeros((n, 4), np.uint8),
+               "distance": np.zeros(n, np.float32), "gradient": np.zeros((n, 3), np.float32)}
+        if priors:
+            out["sem_priors"] = np.zeros((n, nl), np.float32)
+        q = KsgQueryOut(**{k: v.ctypes.data for k, v in out.items()})
+        self._check(self.lib.ksg_query_points(self.handle, n, p.ctypes.data, min_weight, C.byref(q)), "ksg_query_points")
+        return out
+
+    def query_points_device(self, d_xyz: int, n: int, out_ptrs: Dict[str, int], stream: int = 0, min_weight: float = 1e-4):
+        """Enqueue ksg_query_points_device on `stream` (0 = the integrator's own stream): d_xyz and the values of out_ptrs (keys of
+        QUERY_FIELDS; missing keys = not wanted) are raw device pointers.  Returns without waiting."""
+        q = KsgQueryOut(**{k: int(v) for k, v in out_ptrs.items() if v})
+        self._check(self.lib.ksg_query_points_device(self.handle, n, C.c_void_p(d_xyz), min_weight, C.byref(q), C.c_void_p(stream)),
+                    "ksg_query_points_device")
 
     def last_updated_blocks(self) -> np.ndarray:
         n = int(self.lib.ksg_last_updated_blocks(self.handle, 0, None))

@@ -36,6 +36,18 @@ class GpuIntegratorCore {
   // Semantic mesh of the device map (ksg_extract_mesh): triangle soup, per-vertex TsdfVoxel.color and semantic label, blocks in (z, y, x) order
   bool extractMesh(float min_weight, std::vector<float>* vertices, std::vector<uint8_t>* rgba, std::vector<uint8_t>* labels,
                    std::vector<int32_t>* block_index, std::vector<int64_t>* block_first);
+  // Point queries on the device map (ksg_query_points), read-only and without a copy of the map: works in kLazy mode without
+  // syncLayers().  Per point: flags (KSG_QUERY_*), the containing voxel (TsdfVoxel fields, SemanticVoxel label / log-probabilities /
+  // colour; NaN / 0 when its block is not allocated), voxblox's trilinear distance and its gradient (NaN when not valid).
+  struct QueryResult {
+    std::vector<uint8_t> flags;                       // n
+    std::vector<float> tsdf_distance, tsdf_weight;    // n, n
+    std::vector<uint8_t> tsdf_rgba, sem_label;        // 4n, n
+    std::vector<float> sem_priors;                    // n * kTotalNumberOfLabels
+    std::vector<uint8_t> sem_rgba;                    // 4n
+    std::vector<float> distance, gradient;            // n, 3n
+  };
+  bool queryPoints(const vxb::Pointcloud& points_G, float min_weight, QueryResult* result);
   int64_t lastVoxelUpdates() const { return last_voxel_updates_; }
   ksg_integrator* handle() { return handle_; }
 

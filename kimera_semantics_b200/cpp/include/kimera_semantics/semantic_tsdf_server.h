@@ -101,6 +101,12 @@ class SemanticTsdfServer {
     return gpu().extractMesh(min_weight, &mesh->vertices, &mesh->rgba, &mesh->labels, &mesh->block_index, &mesh->block_first);
   }
 
+  // What a planner / scene-graph builder asks the map about points (Layer::getVoxelPtrByCoordinates + Interpolator::getDistance /
+  // getGradient on the host), answered on the device from the device map (ksg_query_points, csrc/ksg_query.cuh): needs no updateLayers().
+  bool queryPoints(const vxb::Pointcloud& points_G, float min_weight, GpuIntegratorCore::QueryResult* result) {
+    return gpu().queryPoints(points_G, min_weight, result);
+  }
+
   vxb::Layer<vxb::TsdfVoxel>* getTsdfLayerPtr() { return tsdf_layer_.get(); }
   vxb::Layer<SemanticVoxel>* getSemanticLayerPtr() { return semantic_layer_.get(); }
   vxb::TsdfIntegratorBase* getIntegratorPtr() { return tsdf_integrator_.get(); }

@@ -307,6 +307,23 @@ bool GpuIntegratorCore::extractMesh(float min_weight, std::vector<float>* vertic
                           &nv, &nb) == KSG_OK;
 }
 
+bool GpuIntegratorCore::queryPoints(const vxb::Pointcloud& points_G, float min_weight, QueryResult* r) {
+  static_assert(sizeof(vxb::Point) == 3 * sizeof(float), "points are passed as packed xyz triples");
+  const size_t n = points_G.size();
+  r->flags.assign(n, 0);
+  r->tsdf_distance.assign(n, 0.0f);
+  r->tsdf_weight.assign(n, 0.0f);
+  r->tsdf_rgba.assign(4 * n, 0);
+  r->sem_label.assign(n, 0);
+  r->sem_priors.assign(n * kTotalNumberOfLabels, 0.0f);
+  r->sem_rgba.assign(4 * n, 0);
+  r->distance.assign(n, 0.0f);
+  r->gradient.assign(3 * n, 0.0f);
+  ksg_query_out out = {r->flags.data(), r->tsdf_distance.data(), r->tsdf_weight.data(), r->tsdf_rgba.data(), r->sem_label.data(),
+                       r->sem_priors.data(), r->sem_rgba.data(), r->distance.data(), r->gradient.data()};
+  return ksg_query_points(handle_, (int64_t)n, n ? reinterpret_cast<const float*>(points_G.data()) : nullptr, min_weight, &out) == KSG_OK;
+}
+
 void GpuIntegratorCore::uploadLayers() {
   vxb::BlockIndexList blocks;
   tsdf_layer_->getAllAllocatedBlocks(&blocks);

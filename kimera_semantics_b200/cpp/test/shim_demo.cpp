@@ -1,9 +1,13 @@
 // Drives the drop-in C++ API exactly the way SemanticTsdfServer does (kimera_semantics_ros/src/semantic_tsdf_server.cpp:58-79):
 // build both layers, SemanticTsdfIntegratorFactory::create(method, ...), then integratePointCloud per frame.
-//   shim_demo <fast|merged|bogus> <frames.bin> <out.bin> [lazy] [--load ckpt] [--save ckpt] [--skip N]
+//   shim_demo <fast|merged|bogus> <frames.bin> <out.bin> [lazy] [--load ckpt] [--save ckpt] [--skip N] [--query in out]
 //     --load: SemanticTsdfServer::loadMap before the first frame; --save: saveMap after the last; --skip: ignore the first N frames
 //     --depth file: instead of the clouds of frames.bin (whose frame count must then be 0) feed depth + label frames:
 //              int32 n, int32 width, int32 height, double K[4], then per frame float T[7], float depth[w*h], uint8 label[w*h]
+//     --query in out: after the last frame (before any layer sync, also in lazy mode) SemanticTsdfServer::queryPoints on the points of
+//              `in` (int32 n, float xyz[3n], world frame; min_weight 1e-4); `out` = the arrays of QueryResult one after the other:
+//              flags[n] u8, tsdf_distance[n] f32, tsdf_weight[n] f32, tsdf_rgba[4n] u8, sem_label[n] u8, sem_priors[n*C] f32,
+//              sem_rgba[4n] u8, distance[n] f32, gradient[3n] f32
 // frames.bin : int32 n_frames, float voxel_size, int32 vps, int32 n_palette, palette n*(r,g,b,a,id), int32 n_dynamic, ids...,
 //              then per frame: int32 n, float T[7], float xyz[3n], uint8 rgba[4n]
 // out.bin    : int32 n_blocks, then per block (sorted z,y,x): int32 idx[3], per voxel: float d, float w, u8 rgba[4], u8 label,
@@ -14,6 +18,7 @@
 #include <cstring>
 #include <fstream>
 #include <vector>
+#include "../../../include/ksg.h"
 #include "kimera_semantics/semantic_tsdf_integrator_factory.h"
 #include "kimera_semantics/semantic_tsdf_integrator_fast.h"
 #include "kimera_semantics/semantic_tsdf_integrator_merged.h"
@@ -39,7 +44,7 @@ int main(int argc, char** argv) {
   vxb::TsdfIntegratorBase::Config config;
   config.default_truncation_distance = 4.0f * voxel_size;  // voxblox_ros
   bool lazy = false;
-  const char *load_path = nullptr, *save_path = nullptr, *depth_path = nullptr;
+  const char *load_path = nullptr, *save_path = nullptr, *depth_path = nullptr, *query_in = nullptr, *query_out = nullptr;
   int skip = 0;
   for (int a = 4; a < argc; ++a) {
     if (std::strcmp(argv[a], "lazy") == 0) lazy = true;
@@ -47,6 +52,7 @@ int main(int argc, char** argv) {
     else if (std::strcmp(argv[a], "--save") == 0 && a + 1 < argc) save_path = argv[++a];
     else if (std::strcmp(argv[a], "--skip") == 0 && a + 1 < argc) skip = std::atoi(argv[++a]);
     else if (std::strcmp(argv[a], "--depth") == 0 && a + 1 < argc) depth_path = argv[++a];
+    else if (std::strcmp(argv[a], "--query") == 0 && a + 2 < argc) { query_in = argv[++a]; query_out = argv[++a]; }
   }
   SemanticTsdfServer::Params params;
   params.tsdf_voxel_size = voxel_size;
@@ -86,6 +92,29 @@ int main(int argc, char** argv) {
                                /*stamp=*/0.2 * fr);
       std::printf("depth frame %d: %lld voxel updates\n", fr, (long long)core->lastVoxelUpdates());
     }
+  }
+  if (query_in) {
+    std::ifstream qf(query_in, std::ios::binary);
+    KSG_CHECK(qf.good()) << "cannot open " << query_in;
+    const int n = rd<int32_t>(qf);
+    vxb::Pointcloud pts(n);
+    qf.read(reinterpret_cast<char*>(pts.data()), sizeof(float) * 3 * n);
+    GpuIntegratorCore::QueryResult q;
+    KSG_CHECK(server.queryPoints(pts, 1e-4f, &q)) << "point query failed";
+    std::ofstream qo(query_out, std::ios::binary);
+    auto put = [&qo](const void* p, size_t bytes) { qo.write(reinterpret_cast<const char*>(p), bytes); };
+    put(q.flags.data(), q.flags.size());
+    put(q.tsdf_distance.data(), 4 * q.tsdf_distance.size());
+    put(q.tsdf_weight.data(), 4 * q.tsdf_weight.size());
+    put(q.tsdf_rgba.data(), q.tsdf_rgba.size());
+    put(q.sem_label.data(), q.sem_label.size());
+    put(q.sem_priors.data(), 4 * q.sem_priors.size());
+    put(q.sem_rgba.data(), q.sem_rgba.size());
+    put(q.distance.data(), 4 * q.distance.size());
+    put(q.gradient.data(), 4 * q.gradient.size());
+    size_t hits = 0;
+    for (uint8_t fl : q.flags) hits += (fl & KSG_QUERY_OBSERVED) ? 1 : 0;
+    std::printf("point query: %d points, %zu in observed voxels%s\n", n, hits, lazy ? " (host layers not synchronised)" : "");
   }
   if (lazy) server.updateLayers();
   {

@@ -25,6 +25,7 @@
 #include "ksg_merge.cuh"
 #include "ksg_eval.cuh"
 #include "ksg_mesh.cuh"
+#include "ksg_query.cuh"
 
 using namespace ksg;
 
@@ -1695,6 +1696,76 @@ int32_t ksg_extract_mesh(ksg_integrator* h, float min_weight, int64_t vertex_cap
   }
 #undef KSG_MESH
   release();
+  return KSG_OK;
+}
+
+namespace {
+// *work = false: the call has nothing to compute (n = 0 or no output wanted) and launches nothing
+int query_args(ksg_integrator* h, int64_t n, const float* xyz, float min_weight, const ksg_query_out* o, bool* work) {
+  if (!h) return KSG_ERR_INVALID_ARGUMENT;
+  if (!o || n < 0 || !(min_weight >= 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "query: NULL out, n < 0 or a NaN / negative min_weight");
+  if (n > 0 && !xyz) return h->fail(KSG_ERR_INVALID_ARGUMENT, "query: NULL points");
+  if (h->dc.shard_count > 1) return h->fail(KSG_ERR_INVALID_ARGUMENT, "query: a sharded integrator holds only its own tiles");
+  *work = n > 0 && (o->flags || o->tsdf_distance || o->tsdf_weight || o->tsdf_rgba || o->sem_label || o->sem_priors || o->sem_rgba ||
+                    o->distance || o->gradient);
+  return KSG_OK;
+}
+void launch_query(ksg_integrator* h, int64_t n, const float* d_xyz, float min_weight, const ksg_query_out& o, cudaStream_t s) {
+  static_assert(sizeof(ksg_query_out) == sizeof(QueryOut), "ksg_query_out layout");
+  QueryOut q{o.flags, o.tsdf_distance, o.tsdf_weight, o.tsdf_rgba, o.sem_label, o.sem_priors, o.sem_rgba, o.distance, o.gradient};
+  const int grid = (int)std::min<int64_t>((n + kQueryThreads - 1) / kQueryThreads, (int64_t)h->sm_count * 8);
+  ++h->n_launches;
+  k_query_points<<<grid, kQueryThreads, 0, s>>>(h->dc, h->map, d_xyz, (long long)n, min_weight, q, (o.flags || o.distance) ? 1 : 0,
+                                                (o.flags || o.gradient) ? 1 : 0);
+}
+}  // namespace
+
+int32_t ksg_query_points(ksg_integrator* h, int64_t n, const float* xyz_G, float min_weight, const ksg_query_out* out) {
+  bool work = false;
+  { const int rca = query_args(h, n, xyz_G, min_weight, out, &work); if (rca) return rca; }
+  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
+  KSG_CUDA(cudaSetDevice(h->device));
+  KSG_CUDA(cudaDeviceSynchronize());
+  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  if (!work) return KSG_OK;
+  const ksg_query_out& o = *out;
+  const size_t N = (size_t)n, C = (size_t)h->dc.C;
+  // one device buffer: points, then every wanted output
+  const size_t sizes[10] = {12 * N, o.flags ? N : 0, o.tsdf_distance ? 4 * N : 0, o.tsdf_weight ? 4 * N : 0, o.tsdf_rgba ? 4 * N : 0,
+                            o.sem_label ? N : 0, o.sem_priors ? 4 * N * C : 0, o.sem_rgba ? 4 * N : 0, o.distance ? 4 * N : 0,
+                            o.gradient ? 12 * N : 0};
+  size_t off[10], total = 0;
+  for (int k = 0; k < 10; ++k) { off[k] = total; total += (sizes[k] + 255) / 256 * 256; }
+  uint8_t* d = nullptr;
+  KSG_CUDA(cudaMalloc((void**)&d, total));
+  auto at = [&](int k) -> void* { return sizes[k] ? (void*)(d + off[k]) : nullptr; };
+  ksg_query_out dq{(uint8_t*)at(1), (float*)at(2), (float*)at(3), (uint8_t*)at(4), (uint8_t*)at(5), (float*)at(6), (uint8_t*)at(7),
+                   (float*)at(8), (float*)at(9)};
+  void* host[10] = {nullptr, o.flags, o.tsdf_distance, o.tsdf_weight, o.tsdf_rgba, o.sem_label, o.sem_priors, o.sem_rgba, o.distance, o.gradient};
+  cudaStream_t s = h->own_stream;
+  cudaError_t e = cudaMemcpyAsync(d, xyz_G, sizes[0], cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) {
+    launch_query(h, n, (const float*)d, min_weight, dq, s);
+    e = cudaGetLastError();
+  }
+  for (int k = 1; k < 10 && e == cudaSuccess; ++k)
+    if (sizes[k]) e = cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  cudaFree(d);
+  if (e != cudaSuccess) return fail(KSG_ERR_CUDA, cudaGetErrorString(e));
+  return KSG_OK;
+}
+
+int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, float min_weight, const ksg_query_out* d_out,
+                                void* cuda_stream) {
+  bool work = false;
+  { const int rca = query_args(h, n, d_xyz_G, min_weight, d_out, &work); if (rca) return rca; }
+  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
+  if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
+  if (!work) return KSG_OK;
+  KSG_CUDA(cudaSetDevice(h->device));
+  launch_query(h, n, d_xyz_G, min_weight, *d_out, cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream);
+  KSG_CUDA(cudaGetLastError());
   return KSG_OK;
 }
 

@@ -246,6 +246,26 @@ struct MapRef {
   int* touched_list;
 };
 
+// Read-side helpers of the map (mesher, point queries): pool slot of a block key (-1: not in the hash) ...
+__device__ __forceinline__ int ht_lookup_slot(const MapRef& m, uint64_t key) {
+  uint32_t pos = mix64(key) & m.ht_mask;
+  for (uint32_t probe = 0; probe <= m.ht_mask; ++probe) {
+    const uint64_t k = m.ht_keys[pos];
+    if (k == key) { const int s = m.ht_slot[pos]; return (s >= 0 && s < m.max_blocks) ? s : -1; }
+    if (k == kEmptyKey) return -1;
+    pos = (pos + 1) & m.ht_mask;
+  }
+  return -1;
+}
+
+// ... and the tile chunk holding voxel (lx, ly, lz) of the block in `slot`, with the voxel's index inside the tile in `vox`
+__device__ __forceinline__ const uint8_t* mesh_voxel_chunk(const DevCfg& cfg, const MapRef& map, int slot, int lx, int ly, int lz, int& vox) {
+  const int ts = cfg.tile_side_log2, tm = cfg.tile_side - 1;
+  const int tile = (lx >> ts) + cfg.tiles_per_side * ((ly >> ts) + cfg.tiles_per_side * (lz >> ts));
+  vox = (lx & tm) + cfg.tile_side * ((ly & tm) + cfg.tile_side * (lz & tm));
+  return map.pool + (uint64_t)slot * cfg.block_stride + (uint64_t)tile * cfg.tile_stride;
+}
+
 __device__ __forceinline__ int ht_find_or_insert_raw(uint64_t* ht_keys, uint32_t ht_mask, int* new_list, int new_cap, uint64_t key, Counters* cnt) {
   uint32_t pos = mix64(key) & ht_mask;
   for (uint32_t probe = 0; probe <= ht_mask; ++probe) {
