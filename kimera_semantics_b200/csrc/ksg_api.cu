@@ -5,10 +5,14 @@
 #include <cub/cub.cuh>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <utility>
 #include <vector>
@@ -33,19 +37,161 @@ namespace {
 
 thread_local std::string g_last_error;
 
+// Every caller names its integrator `h`.
 #define KSG_CUDA(call)                                                                              \
   do {                                                                                              \
     cudaError_t e_ = (call);                                                                        \
     if (e_ != cudaSuccess) {                                                                        \
       char buf_[512];                                                                               \
       snprintf(buf_, sizeof(buf_), "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); \
-      return fail(KSG_ERR_CUDA, buf_);                                                              \
+      return h->fail(KSG_ERR_CUDA, buf_);                                                           \
     }                                                                                               \
   } while (0)
 
 inline int ilog2(int v) { int l = 0; while ((1 << l) < v) ++l; return l; }
 inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 inline int grid_for(long long n, int block) { return (int)std::max<long long>(1, (n + block - 1) / block); }
+
+// f(std::integral_constant<int, NCH>) for the template instance that serves `nch` label chunks (1, 2, 4, otherwise 8)
+template <typename F> auto with_nch(int nch, F&& f) {
+  switch (nch) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    default: return f(std::integral_constant<int, 8>{});
+  }
+}
+// f for every instance, in the order 1, 2, 4, 8; stops at the first non-zero result
+template <typename F> int for_each_nch(F&& f) {
+  for (int nch : {1, 2, 4, 8}) if (const int rc = with_nch(nch, f)) return rc;
+  return 0;
+}
+template <typename F> auto with_tma(bool tma, F&& f) { return tma ? f(std::true_type{}) : f(std::false_type{}); }
+// f(tma, nch) for every (TMA staging, label chunks) instance, TMA first; stops at the first non-zero result
+template <typename F> int for_each_tma_nch(F&& f) {
+  for (const bool tma : {true, false})
+    if (const int rc = with_tma(tma, [&](auto t) { return for_each_nch([&](auto nch) { return f(t, nch); }); })) return rc;
+  return 0;
+}
+
+// Owner of device memory, pinned host memory, streams and events: it remembers what it made and releases what it still holds
+// in reverse order when it is destroyed.  The caller selects the device.
+class Resources {
+ public:
+  Resources() = default;
+  Resources(const Resources&) = delete;
+  Resources& operator=(const Resources&) = delete;
+  ~Resources() { for (auto it = held_.rbegin(); it != held_.rend(); ++it) destroy(*it); }
+
+  // (the call is made before *p is read: keep() takes the result, not the call)
+  template <typename Tp> cudaError_t device(Tp** p, size_t count) { return alloc(p, count, kDevice); }
+  template <typename Tp> cudaError_t pinned(Tp** p, size_t count) { return alloc(p, count, kPinned); }
+  cudaError_t stream(cudaStream_t* s) {
+    const cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+    return keep(e, kStream, (void*)*s);
+  }
+  cudaError_t stream(cudaStream_t* s, int priority) {
+    const cudaError_t e = cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, priority);
+    return keep(e, kStream, (void*)*s);
+  }
+  cudaError_t event(cudaEvent_t* ev, unsigned flags) {
+    const cudaError_t e = cudaEventCreateWithFlags(ev, flags);
+    return keep(e, kEvent, (void*)*ev);
+  }
+
+  // Releases one allocation before the owner goes (nullptr: nothing to do).
+  void release(void* p) {
+    if (!p) return;
+    for (size_t i = held_.size(); i-- > 0;)
+      if (held_[i].p == p) { destroy(held_[i]); held_.erase(held_.begin() + (ptrdiff_t)i); return; }
+  }
+  // A buffer that grows: *p is released and replaced by `count` fresh elements (the contents are not kept).  *cap records the
+  // new capacity, or 0 when the allocation fails.
+  template <typename Tp, typename Cap> cudaError_t regrow(Tp** p, Cap* cap, size_t count) { return replace(p, cap, count, kDevice); }
+  template <typename Tp, typename Cap> cudaError_t regrow_pinned(Tp** p, Cap* cap, size_t count) { return replace(p, cap, count, kPinned); }
+
+ private:
+  enum Kind { kDevice, kPinned, kStream, kEvent };
+  struct Item { Kind kind; void* p; };
+  template <typename Tp> cudaError_t alloc(Tp** p, size_t count, Kind kind) {
+    const size_t bytes = std::max<size_t>(count, 1) * sizeof(Tp);
+    const cudaError_t e = kind == kPinned ? cudaMallocHost((void**)p, bytes) : cudaMalloc((void**)p, bytes);
+    return keep(e, kind, (void*)*p);
+  }
+  template <typename Tp, typename Cap> cudaError_t replace(Tp** p, Cap* cap, size_t count, Kind kind) {
+    release(*p); *p = nullptr; *cap = 0;
+    const cudaError_t e = alloc(p, count, kind);
+    if (e == cudaSuccess) *cap = (Cap)count;
+    return e;
+  }
+  cudaError_t keep(cudaError_t e, Kind kind, void* p) {
+    if (e == cudaSuccess && p) held_.push_back(Item{kind, p});
+    return e;
+  }
+  static void destroy(const Item& it) {
+    switch (it.kind) {
+      case kDevice: cudaFree(it.p); break;
+      case kPinned: cudaFreeHost(it.p); break;
+      case kStream: cudaStreamDestroy(static_cast<cudaStream_t>(it.p)); break;
+      case kEvent: cudaEventDestroy(static_cast<cudaEvent_t>(it.p)); break;
+    }
+  }
+  std::vector<Item> held_;
+};
+
+// Development knobs (environment), read once when an integrator is created.  They select experiments and shapes that were
+// measured against the defaults; ksg_create applies each one only where it mattered before (see there).
+//
+// KSG_HOT_KERNEL=1 and KSG_EMIT_WARP=1 were both slower than what they were meant to replace when they were written (the hot
+// voxels' critical path is the TSDF weight recurrence, which a producer / consumer ring does not shorten; the warp-wide ray walk
+// costs more in rank searches than the scattered stores it saves) - kept as opt-in experiments.
+// The short-segment kernel is capped at short_ctas CTAs per SM through a dynamic shared-memory reservation so that a CTA of the
+// long-segment kernel (128 registers per thread) always finds room beside it - otherwise the two kernels run back to back.
+// short_t_ctas: the frame is bound by the long-segment kernel (128 registers per thread); whatever the short kernel takes from it
+// costs more than it gains.  Re-measured on an H100 80GB HBM3 (400 W, merged2, bench.py --quick, two alternating passes):
+// KSG_SHORT_T_CTAS 1 -> 164 frames/s, 2 -> 181-182, 3 -> 171-173, 4 -> 177-178; KSG_LONG_THREADS=128 172-176,
+// KSG_DEEP_THREADS=64 180-182, KSG_LONG_SERIAL=0 176-178 - the defaults below stay.
+struct Knobs {
+  bool tile_apply = false;        // KSG_MERGED_TILE_APPLY=1: merged uses the tile kernel instead of the per-voxel kernels
+  bool short_thread = true;       // KSG_SHORT_THREAD=0: merged, C <= 32: the warp-per-voxel short kernel instead of k_voxel_apply_short_t
+  int long_len = 0;               // KSG_LONG_LEN: records from which a voxel is long under k_voxel_apply_short_t (0: kLongLenThread)
+  bool l2_persist = false;        // KSG_L2_PERSIST=1: experiment, the (L * freq) rows persist in L2
+  bool hot_kernel = false;        // KSG_HOT_KERNEL=1
+  int long_threads = 256;         // KSG_LONG_THREADS: 64, 128 or 256
+  int long_grid = 0;              // KSG_LONG_GRID (0: one CTA per SM)
+  bool deep_hot = true;           // KSG_DEEP_HOT=0: the hot voxels do not get the deep-pipeline instance of k_voxel_apply_long
+  bool long_serial = true;        // KSG_LONG_SERIAL=0: the non-hot long segments (0.3 ms standalone) run beside the short kernel
+  int deep_threads = 128;         // KSG_DEEP_THREADS: block size of the hot-voxel instance (32, 64, 128 or 256), one warp per chain
+  int short_t_ctas = 2;           // KSG_SHORT_T_CTAS: CTAs per SM of k_voxel_apply_short_t, 1 to 8
+  int short_ctas = 3;             // KSG_SHORT_CTAS: CTAs per SM of k_voxel_apply_short, 1 to 6
+  bool emit_warp = false;         // KSG_EMIT_WARP=1
+  int solve_threads = kSolveThreads;   // KSG_SOLVE_THREADS: 256, 512 or 1024
+  int solve_ctas_per_sm = INT_MAX;     // KSG_SOLVE_CTAS_PER_SM, at least 1 and at most what the occupancy allows
+  bool profile_marks_only = false;     // KSG_PROFILE_MARKS_ONLY=1: fast, the solve kernel's phase marks without its per-ray probes
+};
+
+Knobs read_knobs() {
+  Knobs k;
+  auto env = [](const char* name, int* v) { const char* e = std::getenv(name); if (e) *v = std::atoi(e); return e != nullptr; };
+  int v = 0;
+  if (env("KSG_MERGED_TILE_APPLY", &v) && v != 0) k.tile_apply = true;
+  if (env("KSG_SHORT_THREAD", &v)) k.short_thread = v != 0;
+  if (env("KSG_LONG_LEN", &v)) k.long_len = std::max(kLongLen, std::min(1 << 20, v));
+  if (env("KSG_L2_PERSIST", &v)) k.l2_persist = v != 0;
+  if (env("KSG_HOT_KERNEL", &v)) k.hot_kernel = v != 0;
+  if (env("KSG_LONG_THREADS", &v) && (v == 64 || v == 128 || v == 256)) k.long_threads = v;
+  if (env("KSG_LONG_GRID", &v)) k.long_grid = std::max(1, v);
+  if (env("KSG_DEEP_HOT", &v)) k.deep_hot = v != 0;
+  if (env("KSG_LONG_SERIAL", &v)) k.long_serial = v != 0;
+  if (env("KSG_DEEP_THREADS", &v) && (v == 32 || v == 64 || v == 128 || v == 256)) k.deep_threads = v;
+  if (env("KSG_SHORT_T_CTAS", &v)) k.short_t_ctas = std::max(1, std::min(8, v));
+  if (env("KSG_SHORT_CTAS", &v)) k.short_ctas = std::max(1, std::min(6, v));
+  if (env("KSG_EMIT_WARP", &v)) k.emit_warp = v != 0;
+  if (env("KSG_SOLVE_THREADS", &v) && (v == 256 || v == 512 || v == 1024)) k.solve_threads = v;
+  if (env("KSG_SOLVE_CTAS_PER_SM", &v)) k.solve_ctas_per_sm = v;
+  if (env("KSG_PROFILE_MARKS_ONLY", &v)) k.profile_marks_only = v != 0;
+  return k;
+}
 
 }  // namespace
 
@@ -133,7 +279,7 @@ struct ksg_integrator {
   long long rec_cap = 0;
   long long* tile_begin = nullptr;
   long long tile_cap = 0;
-  void* cub_temp = nullptr;
+  uint8_t* cub_temp = nullptr;
   size_t cub_temp_bytes = 0;
 
   // host staging (pinned) + device input buffers for the host-buffer entry points
@@ -156,7 +302,7 @@ struct ksg_integrator {
   int *tile_cnt = nullptr, *tile_slot = nullptr;
   TileDesc* tile_list = nullptr;
   int solve_grid = 0, apply_fast_smem = 0;
-  int solve_threads = kSolveThreads; // tuning knobs (environment): KSG_SOLVE_THREADS, KSG_SOLVE_CTAS_PER_SM
+  int solve_threads = 0;             // Knobs
   RayRec* rayrec = nullptr;
   int* wl = nullptr;                 // [3][max_points] per-ray listed sweep, two scan lists
   int *mixed_list = nullptr, *m_list = nullptr, *blk_run = nullptr;
@@ -189,26 +335,15 @@ struct ksg_integrator {
   VoxelQueues vq{};
   cudaStream_t aux_stream = nullptr, aux_stream2 = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_join2 = nullptr;
-  // both were slower than what they were meant to replace when they were written (the hot
-  // voxels' critical path is the TSDF weight recurrence, which a producer / consumer ring does not shorten; the warp-wide ray walk costs
-  // more in rank searches than the scattered stores it saves) - kept as opt-in experiments: KSG_HOT_KERNEL=1, KSG_EMIT_WARP=1
+  // shape and experiments of the per-voxel kernels: development knobs (Knobs), set by ksg_create for the per-voxel apply only
   bool hot_kernel = false;
   bool emit_warp = false;
-  // shape of the two per-voxel kernels (environment: KSG_LONG_THREADS, KSG_LONG_GRID, KSG_SHORT_CTAS): the short-segment kernel is
-  // capped at short_ctas CTAs per SM through a dynamic shared-memory reservation so that a CTA of the long-segment kernel (128
-  // registers per thread) always finds room beside it - otherwise the two kernels run back to back
-  int long_threads = 256, long_grid = 0, short_ctas = 3, short_smem = 0;
+  int long_threads = 0, long_grid = 0, short_ctas = 0, short_smem = 0;
   bool short_thread = false;         // merged, C <= 32: k_voxel_apply_short_t
-  // the non-hot long segments (0.3 ms standalone) run behind the short kernel on its stream instead of beside it (KSG_LONG_SERIAL=0:
-  // beside it)
-  bool long_serial = true;
-  int deep_threads = 128;            // block size of the hot-voxel instance (KSG_DEEP_THREADS): one warp per chain, 4 warps per CTA
-  bool deep_hot = true;              // merged, C <= 32: the hot voxels go to the deep-pipeline instance of k_voxel_apply_long (KSG_DEEP_HOT=0: off)
-  // its CTAs per SM (KSG_SHORT_T_CTAS).  The frame is bound by the long-segment kernel (128 registers per thread); whatever the
-  // short kernel takes from it costs more than it gains.  Re-measured on an H100 80GB HBM3 (400 W, merged2, bench.py --quick, two
-  // alternating passes): 1 -> 164 frames/s, 2 -> 181-182, 3 -> 171-173, 4 -> 177-178; KSG_LONG_THREADS=128 172-176,
-  // KSG_DEEP_THREADS=64 180-182, KSG_LONG_SERIAL=0 176-178 - the defaults below stay
-  int short_t_ctas = 2;
+  bool long_serial = false;
+  int deep_threads = 0;
+  bool deep_hot = false;             // merged, C <= 32: the hot voxels go to the deep-pipeline instance of k_voxel_apply_long
+  int short_t_ctas = 0;
   int hot_smem = 0;
 
   long long* tile_debug = nullptr;  // optional per-tile (records, cycles) trace
@@ -218,12 +353,15 @@ struct ksg_integrator {
 
   // profiling
   bool profiling = false;
-  bool profile_marks_only = false;   // fast (KSG_PROFILE_MARKS_ONLY=1): the solve kernel's phase marks without its per-ray probes
+  bool profile_marks_only = false;   // fast (Knobs): the solve kernel's phase marks without its per-ray probes
   cudaEvent_t ev[KSG_NUM_PHASES + 1] = {};
   double phase_ms[KSG_NUM_PHASES] = {};
   int64_t prof_frames = 0;
   int64_t n_launches = 0, n_libcalls = 0;
 
+  Resources res;                     // every device / pinned buffer, stream and event above that is not an alias into another
+
+  ~ksg_integrator() { cudaSetDevice(device); }   // then `res` releases
   int fail(int code, const char* msg) { err = msg; g_last_error = msg; return code; }
 };
 
@@ -255,44 +393,6 @@ int validate(const ksg_config* c, std::string& why) {
   return KSG_OK;
 }
 
-template <typename Tp>
-cudaError_t dmalloc(Tp** p, size_t count) { return cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(Tp)); }
-
-void free_all(ksg_integrator* h) {
-  cudaSetDevice(h->device);
-  void* ptrs[] = {h->map.ht_keys, h->map.ht_slot, h->map.new_list, h->map.pool, h->map.slot_key, h->map.touched_stamp,
-                  h->map.touched_list, h->d_luts, h->d_cnt, h->pt_pC, h->pt_pG, h->pt_label, h->pt_flags, h->pt_color, h->pt_key,
-                  h->flags8, h->pix_list, h->point_of_seq, h->sq_keys, h->sq_keys_out, h->iota,
-                  h->start_next, h->start_min, h->clear_ff, h->clear_00, h->start_table, h->cast_seq, h->ray_param, h->ray_label, h->ray_flags,
-                  h->ray_color, h->nsteps, h->ray_state, h->ext_off, h->o3.cand, h->o3.bkt, h->o3.ovf, h->o3.stamp_max, h->o3.table, h->ks_sorted, h->seq_sorted, h->bstart, h->bundle_f, h->hist,
-                  h->tmp, h->tmp4, h->b_key, h->b_base, h->bord_hash, h->bord_scratch, h->d_scan_tot, h->bundle_f2, h->d_hot_segs, h->d_hot_counts, h->d_hot_chunk_seg, h->d_hot_guess, h->d_hot_sums,
-                  h->d_hot_tables, h->d_hot_prior, h->d_hot_same, h->tile_debug, h->d_fc, h->blk_cnt, h->blk_off, h->warp_cnt, h->warp_off, h->seq_of_i, h->keys32,
-                  h->tile_cnt, h->tile_slot, h->tile_list, h->rayrec, h->wl, h->mixed_list, h->m_list, h->blk_run, h->d_log_head, h->d_log_prior, h->vq.long_items, h->vq.counters, h->rec_a, h->rec_b, h->tile_begin, h->cub_temp, h->d_in, h->d_exp, h->d_exp_slots};
-  for (void* p : ptrs) if (p) cudaFree(p);
-  if (h->h_cnt_base) cudaFreeHost(h->h_cnt_base);
-  if (h->h_log_head) cudaFreeHost(h->h_log_head);
-  if (h->h_log_prior) cudaFreeHost(h->h_log_prior);
-  if (h->h_fc_base) cudaFreeHost(h->h_fc_base);
-  for (int i = 0; i < 2; ++i) {
-    if (h->ev_frame_s[i]) cudaEventDestroy(h->ev_frame_s[i]);
-    if (h->ev_copy[i]) cudaEventDestroy(h->ev_copy[i]);
-    if (h->ev_free[i]) cudaEventDestroy(h->ev_free[i]);
-    if (h->d_in2[i]) cudaFree(h->d_in2[i]);
-    if (h->h_stage2[i]) cudaFreeHost(h->h_stage2[i]);
-  }
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
-  if (h->ev_join2) cudaEventDestroy(h->ev_join2);
-  if (h->aux_stream2) cudaStreamDestroy(h->aux_stream2);
-  if (h->aux_stream) cudaStreamDestroy(h->aux_stream);
-  if (h->h_stage) cudaFreeHost(h->h_stage);
-  if (h->h_hot_segs) cudaFreeHost(h->h_hot_segs);
-  if (h->h_hot_chunk_seg) cudaFreeHost(h->h_hot_chunk_seg);
-  for (auto& e : h->ev) if (e) cudaEventDestroy(e);
-  if (h->own_stream) cudaStreamDestroy(h->own_stream);
-}
-
 __global__ void k_iota(uint32_t* p, int n) { const int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = (uint32_t)i; }
 
 // "sorted" integration order (voxblox SortedThreadSafeIndex, A.3): key = squared norm of the point
@@ -311,7 +411,6 @@ __global__ void k_sqnorm(FrameIn in, const Counters* cnt, int capacity, uint32_t
 }
 
 int reset_map(ksg_integrator* h, cudaStream_t s) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaMemsetAsync(h->map.ht_keys, 0xFF, sizeof(uint64_t) * h->ht_cap, s));
   KSG_CUDA(cudaMemsetAsync(h->map.ht_slot, 0xFF, sizeof(int) * h->ht_cap, s));
   KSG_CUDA(cudaMemsetAsync(h->map.touched_stamp, 0, sizeof(int) * h->ht_cap, s));
@@ -354,7 +453,6 @@ struct InputDesc {
 };
 
 int fetch_counters(ksg_integrator* h, cudaStream_t s) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaMemcpyAsync(h->h_cnt, h->d_cnt, sizeof(Counters), cudaMemcpyDeviceToHost, s));
   KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
@@ -371,12 +469,10 @@ const char* err_text(int e) {
   }
 }
 
-// hot_voxel_mode = 1: finish the log-probability rows of the frame's hot voxels ahead of the tile kernel (ksg_hot.cuh).
+// hot_voxel_mode = 1: finish the log-probability rows of the frame's hot voxels ahead of the apply kernels (ksg_hot.cuh).
 // Returns the number of hot segments (0: nothing to do) through *n_hot.
-int hot_voxel_prepass(ksg_integrator* h, cudaStream_t s, const Xform& T, const float4* bundle_param, long long n_records, int* n_hot) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
+int hot_voxel_rows(ksg_integrator* h, cudaStream_t s, const Xform& T, const float4* bundle_param, long long n_records, int* n_hot) {
   const DevCfg& dc = h->dc;
-  *n_hot = 0;
   KSG_CUDA(cudaMemsetAsync(h->d_hot_counts, 0, sizeof(int), s));
   ++h->n_launches;
   k_hot_find<<<grid_for(n_records, 256), 256, 0, s>>>(dc, h->map, h->rec_b, n_records, h->d_hot_segs, h->d_hot_counts);
@@ -420,6 +516,15 @@ int hot_voxel_prepass(ksg_integrator* h, cudaStream_t s, const Xform& T, const f
   *n_hot = kept;
   return KSG_OK;
 }
+// The pre-pass, with `src` pointed at its results for the apply kernels.
+int hot_voxel_prepass(ksg_integrator* h, cudaStream_t s, const Xform& T, long long n_records, ApplySrc* src, int* n_hot) {
+  *n_hot = 0;
+  const int rc = hot_voxel_rows(h, s, T, src->param, n_records, n_hot);
+  if (rc) return rc;
+  src->hot_segs = h->d_hot_segs; src->hot_prior = h->d_hot_prior; src->n_hot = *n_hot; src->hot_thresh = kHotThresh;
+  src->hot_tsdf_same = (h->cfg.hot_voxel_mode == 2) ? h->d_hot_same : nullptr;
+  return KSG_OK;
+}
 
 
 void fill_stats(ksg_integrator* h, ksg_frame_stats* stats) {
@@ -435,10 +540,32 @@ void fill_stats(ksg_integrator* h, ksg_frame_stats* stats) {
   stats->fixpoint_iterations = h->h_fc ? h->h_fc->sweeps_last : 0;
 }
 
+// The end of every frame, once its counters are on the host: the map's size mirrored, and a device-side error turned into
+// the integrator's deferred status.
+void mirror_counters(ksg_integrator* h) {
+  h->num_blocks = h->h_cnt->pool_count;
+  h->last_blocks_touched = h->h_cnt->n_blocks_touched;
+}
+int device_error(ksg_integrator* h) {
+  const int dev_err = h->h_cnt->err;
+  if (dev_err) {
+    h->deferred_status = dev_err;  // the map may be inconsistent from here on
+    return h->fail(dev_err, err_text(dev_err));
+  }
+  return KSG_OK;
+}
+// The synchronous epilogue of the map-merge entries
+int finish_sync(ksg_integrator* h, cudaStream_t s) {
+  KSG_CUDA(cudaGetLastError());
+  const int rc = fetch_counters(h, s);
+  if (rc) return rc;
+  mirror_counters(h);
+  return device_error(h);
+}
+
 // Completes the OLDEST frame whose counters are still in flight (fast): waits for its counter copy, mirrors the
 // counters on the host and reports a device-side error.
 int finish_oldest(ksg_integrator* h, ksg_frame_stats* stats) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   if (h->n_pend <= 0) return KSG_OK;
   const int slot = h->pend[0];
   h->pend[0] = h->pend[1];
@@ -446,8 +573,7 @@ int finish_oldest(ksg_integrator* h, ksg_frame_stats* stats) {
   KSG_CUDA(cudaEventSynchronize(h->ev_frame_s[slot]));
   h->h_cnt = h->h_cnt_base + slot;
   if (h->h_fc_base) h->h_fc = h->h_fc_base + slot;
-  h->num_blocks = h->h_cnt->pool_count;
-  h->last_blocks_touched = h->h_cnt->n_blocks_touched;
+  mirror_counters(h);
   if (h->profiling && h->h_fc) {
     // events: 0 frame start, 1 before the solve kernel, 2 after it, 3 after the tile kernel; the solve kernel's own phases come from
     // the clock64 marks block 0 left in FastCounters::timeline
@@ -470,12 +596,7 @@ int finish_oldest(ksg_integrator* h, ksg_frame_stats* stats) {
     h->prof_frames += 1;
   }
   if (stats) fill_stats(h, stats);
-  const int dev_err = h->h_cnt->err;
-  if (dev_err) {
-    h->deferred_status = dev_err;  // the map may be inconsistent from here on
-    return fail(dev_err, err_text(dev_err));
-  }
-  return KSG_OK;
+  return device_error(h);
 }
 // Completes every outstanding frame; `stats` receives the newest frame's counters.
 int finish_frame(ksg_integrator* h, ksg_frame_stats* stats) {
@@ -488,7 +609,6 @@ int finish_frame(ksg_integrator* h, ksg_frame_stats* stats) {
 
 // fast: ApproxHashSet resets (fast.cpp:165-170, A.4), once per frame before any point is looked at
 int advance_sets(ksg_integrator* h, cudaStream_t s) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   if ((++h->reset_counter) >= h->cfg.clear_checks_every_n_frames) {
     h->reset_counter = 0;
     if (++h->set_offset >= 10000) {
@@ -503,7 +623,6 @@ int advance_sets(ksg_integrator* h, cudaStream_t s) {
 // `fast` frame driver: five launches, no host read-back inside the frame (ksg_fast.cuh).
 int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, const Xform& T, int cap, cudaStream_t s,
                    ksg_frame_stats* stats) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   const bool sorted = h->cfg.integration_order_mode == KSG_ORDER_SORTED;
   { const int rcs = advance_sets(h, s); if (rcs) return rcs; }
   FastFrame f{};
@@ -576,15 +695,11 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
     const int ctas_per_sm = std::max(1, std::min(8, (int)(220 * 1024 / std::max(1, h->apply_fast_smem + 1024))));
     const int grid = h->sm_count * ctas_per_sm;
     ++h->n_launches;
-#define KSG_LAUNCH_FAST(TMA, NCH) k_tile_apply_fast<TMA, NCH><<<grid, 512, h->apply_fast_smem, s>>>(f, src)
-    if (h->use_tma) {
-      switch (h->apply_nch) { case 1: KSG_LAUNCH_FAST(true, 1); break; case 2: KSG_LAUNCH_FAST(true, 2); break;
-                              case 4: KSG_LAUNCH_FAST(true, 4); break; default: KSG_LAUNCH_FAST(true, 8); break; }
-    } else {
-      switch (h->apply_nch) { case 1: KSG_LAUNCH_FAST(false, 1); break; case 2: KSG_LAUNCH_FAST(false, 2); break;
-                              case 4: KSG_LAUNCH_FAST(false, 4); break; default: KSG_LAUNCH_FAST(false, 8); break; }
-    }
-#undef KSG_LAUNCH_FAST
+    with_tma(h->use_tma, [&](auto tma) {
+      with_nch(h->apply_nch, [&](auto nch) {
+        k_tile_apply_fast<decltype(tma)::value, decltype(nch)::value><<<grid, 512, h->apply_fast_smem, s>>>(f, src);
+      });
+    });
   }
   if (h->profiling) cudaEventRecord(h->ev[3], s);
   KSG_CUDA(cudaGetLastError());
@@ -604,51 +719,29 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   return KSG_OK;
 }
 
-int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaStream_t s, ksg_frame_stats* stats) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
-  if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
-  if (in.n > h->cap_points) return fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");
-  if (in.n == 0 && h->n_pend > 0) { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
-  KSG_CUDA(cudaSetDevice(h->device));
+// `merged` frame: what one stage of the driver hands to the next
+struct MergedFrame {
+  const InputDesc& in;
+  FrameIn fin;
+  Xform T;
+  int cap;                 // host upper bound of the point count
+  cudaStream_t s;
+  long long n_records = 0;
+  int n_hot = 0;           // hot segments of the pre-pass (hot_voxel_mode >= 1)
+  ApplySrc src{};
+};
+
+// Bundling: the points classified and grouped into bundles (one ray each), the bundles' record ranges; ends with the counters
+// on the host.
+int merged_bundles(ksg_integrator* h, MergedFrame& m) {
   const DevCfg& dc = h->dc;
-  const bool fast = h->cfg.integrator_type == KSG_INTEGRATOR_FAST;
-  const int cap = (int)in.n;  // host upper bound of the point count
-  const int B = 256;
-  Xform T{T_host[0], T_host[1], T_host[2], T_host[3], T_host[4], T_host[5], T_host[6]};
-  h->frame_stamp += 1;
-
-  if (cap == 0) {
-    if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->blocks_allocated = h->num_blocks; }
-    if (fast) { const int rcs = advance_sets(h, s); if (rcs) return rcs; }   // the sets are reset even for an empty frame
-    else h->merged_log_count = 0;
-    h->last_blocks_touched = 0;
-    return KSG_OK;
-  }
-
-  FrameIn fin{};
-  fin.xyz = in.d_xyz; fin.rgba = in.d_rgba; fin.labels = in.d_labels;
-  fin.depth = in.d_depth; fin.label_img = in.d_label_img; fin.pix_list = h->pix_list;
-  fin.point_of_seq = nullptr;
-  fin.width = in.width;
-  fin.cx = (float)in.K[2]; fin.cy = (float)in.K[3];   // depth_map_to_pointcloud.h:222-223 float center = model_.cx()
-  if (in.d_depth) {  // depth_map_to_pointcloud.h:228-230: float constant = unit_scaling / f  (double division)
-    fin.constant_x = (float)(in.unit_scaling / in.K[0]);
-    fin.constant_y = (float)(in.unit_scaling / in.K[1]);
-  }
-  fin.z_scale = in.z_scale;
-  fin.color_img = in.d_color_img;
-  fin.freespace = in.freespace;
-  if (fast) return integrate_fast(h, in, fin, T, cap, s, stats);
-
-  // merged
-  h->merged_log_count = 0;
-  bool log_written = false;
-  if (h->profiling) cudaEventRecord(h->ev[0], s);
+  const int cap = m.cap, B = 256;
+  cudaStream_t s = m.s;
   ++h->n_launches;
-  k_frame_reset<<<1, 1, 0, s>>>(h->d_cnt, in.d_depth ? 0 : cap);
-  if (in.d_depth) {
+  k_frame_reset<<<1, 1, 0, s>>>(h->d_cnt, m.in.d_depth ? 0 : cap);
+  if (m.in.d_depth) {
     ++h->n_launches;
-    k_depth_flags<<<grid_for(cap, B), B, 0, s>>>(in.d_depth, cap, h->flags8);
+    k_depth_flags<<<grid_for(cap, B), B, 0, s>>>(m.in.d_depth, cap, h->flags8);
     size_t tb = h->cub_temp_bytes;
     ++h->n_libcalls;
     KSG_CUDA(cub::DeviceSelect::Flagged(h->cub_temp, tb, cub::CountingInputIterator<int>(0), h->flags8, h->pix_list,
@@ -656,19 +749,15 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
   }
   if (h->cfg.integration_order_mode == KSG_ORDER_SORTED) {
     ++h->n_launches;
-    k_sqnorm<<<grid_for(cap, B), B, 0, s>>>(fin, h->d_cnt, cap, h->sq_keys);
+    k_sqnorm<<<grid_for(cap, B), B, 0, s>>>(m.fin, h->d_cnt, cap, h->sq_keys);
     size_t tb = h->cub_temp_bytes;
     ++h->n_libcalls;
     KSG_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_temp, tb, h->sq_keys, h->sq_keys_out, h->iota, (uint32_t*)h->point_of_seq,
                                              cap, 0, 32, s));
-    fin.point_of_seq = h->point_of_seq;
+    m.fin.point_of_seq = h->point_of_seq;
   }
-
-  long long n_records = 0;
-  int64_t last_hot_voxels = 0;
-  ApplySrc src{};
   ++h->n_launches;
-  k_classify<<<grid_for(cap, B), B, 0, s>>>(dc, T, fin, h->d_luts, cap, h->d_cnt, h->pt_pC, h->pt_pG, h->pt_label,
+  k_classify<<<grid_for(cap, B), B, 0, s>>>(dc, m.T, m.fin, h->d_luts, cap, h->d_cnt, h->pt_pC, h->pt_pG, h->pt_label,
                                             h->pt_flags, h->pt_color, h->pt_key);
   if (h->profiling) cudaEventRecord(h->ev[1], s);
   {
@@ -694,166 +783,172 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
     bundle_heads = h->bundle_f2;
   }
   ++h->n_launches;
-  k_bundle_merge<<<h->sm_count * 8, 256, 0, s>>>(dc, T, h->d_cnt, bundle_heads, h->bstart, h->ks_sorted, h->seq_sorted, cap, h->pt_pC,
+  k_bundle_merge<<<h->sm_count * 8, 256, 0, s>>>(dc, m.T, h->d_cnt, bundle_heads, h->bstart, h->ks_sorted, h->seq_sorted, cap, h->pt_pC,
                                                  h->pt_label, h->hist, h->ray_param, h->ray_flags, h->b_key, h->nsteps);
   ++h->n_launches;
   k_bundle_scan<<<kBordCluster, kBordThreads, 0, s>>>(h->d_cnt, h->nsteps, h->b_base, h->rec_cap, h->d_scan_tot);
-  int rc = fetch_counters(h, s);
-  if (rc) return rc;
-  if (h->profiling) cudaEventRecord(h->ev[2], s);
-  if (!h->h_cnt->err) {
-    const int nb = std::max(1, h->h_cnt->n_cast);
-    n_records = (long long)h->h_cnt->n_records;
-    ++h->n_launches;
-    k_bundle_loglik<<<grid_for((long long)(nb + 1) * dc.C, B), B, 0, s>>>(dc, h->d_cnt, h->hist, h->tmp, h->tmp4);
-    ++h->n_launches;
-    if (h->emit_warp)
-      k_emit_merged_warp<<<h->sm_count * 8, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->ray_param, h->ray_flags, h->b_key, h->nsteps, h->b_base,
-                                                         h->ks_sorted, cap, h->rec_a);
-    else
-    k_emit_merged<<<grid_for(nb, 128), 128, 0, s>>>(dc, T, h->d_cnt, h->map, h->ray_param, h->ray_flags, h->b_key, h->nsteps,
-                                                    h->b_base, h->ks_sorted, cap, h->rec_a);
-  }
-  src.param = h->ray_param; src.label = nullptr; src.color = nullptr; src.tmp = h->tmp; src.tmp4 = h->tmp4;
+  return fetch_counters(h, s);
+}
 
-  if (h->profiling) cudaEventRecord(h->ev[3], s);
-  int dev_err = h->h_cnt->err;
-  bool did_apply = false;
-  if (!dev_err && n_records > 0) {
-    // order the update records by (tile, voxel, order): per-voxel application order = reference order
-    size_t tb = h->cub_temp_bytes;
-    ++h->n_libcalls;
-    // significant key bits: [order 23][voxel 9][tile key < ht_cap * tiles_per_block]
-    int end_bit = 32;
-    while (end_bit < 64 && (1ull << (end_bit - 32)) < (unsigned long long)h->ht_cap * (unsigned long long)dc.tiles_per_block) ++end_bit;
-    // the records were laid out by (bundle rank, step), so a stable sort on the voxel bits [23, end) keeps the rank order
-    KSG_CUDA(cub::DeviceRadixSort::SortKeys(h->cub_temp, tb, h->rec_a, h->rec_b, n_records, kRecOrdBits, end_bit, s));
-    if (h->profiling) cudaEventRecord(h->ev[4], s);
+// The bundles' log-likelihood rows and their update records
+void merged_emit(ksg_integrator* h, MergedFrame& m) {
+  const DevCfg& dc = h->dc;
+  const int B = 256;
+  cudaStream_t s = m.s;
+  const int nb = std::max(1, h->h_cnt->n_cast);
+  m.n_records = (long long)h->h_cnt->n_records;
+  ++h->n_launches;
+  k_bundle_loglik<<<grid_for((long long)(nb + 1) * dc.C, B), B, 0, s>>>(dc, h->d_cnt, h->hist, h->tmp, h->tmp4);
+  ++h->n_launches;
+  if (h->emit_warp)
+    k_emit_merged_warp<<<h->sm_count * 8, 256, 0, s>>>(dc, m.T, h->d_cnt, h->map, h->ray_param, h->ray_flags, h->b_key, h->nsteps, h->b_base,
+                                                       h->ks_sorted, m.cap, h->rec_a);
+  else
+    k_emit_merged<<<grid_for(nb, 128), 128, 0, s>>>(dc, m.T, h->d_cnt, h->map, h->ray_param, h->ray_flags, h->b_key, h->nsteps,
+                                                    h->b_base, h->ks_sorted, m.cap, h->rec_a);
+}
+
+// The update records in (tile, voxel, order) order: per-voxel application order = reference order; then the frame's new blocks
+int merged_sort_records(ksg_integrator* h, MergedFrame& m) {
+  const DevCfg& dc = h->dc;
+  cudaStream_t s = m.s;
+  size_t tb = h->cub_temp_bytes;
+  ++h->n_libcalls;
+  // significant key bits: [order 23][voxel 9][tile key < ht_cap * tiles_per_block]
+  int end_bit = 32;
+  while (end_bit < 64 && (1ull << (end_bit - 32)) < (unsigned long long)h->ht_cap * (unsigned long long)dc.tiles_per_block) ++end_bit;
+  // the records were laid out by (bundle rank, step), so a stable sort on the voxel bits [23, end) keeps the rank order
+  KSG_CUDA(cub::DeviceRadixSort::SortKeys(h->cub_temp, tb, h->rec_a, h->rec_b, m.n_records, kRecOrdBits, end_bit, s));
+  if (h->profiling) cudaEventRecord(h->ev[4], s);
+  ++h->n_launches;
+  k_block_init<<<h->sm_count * 4, 256, 0, s>>>(dc, h->d_cnt, h->map);
+  return KSG_OK;
+}
+
+// Per-voxel update (ksg_voxel.cuh): segment heads -> two queues; the long and the short kernel run concurrently
+int merged_apply_voxels(ksg_integrator* h, MergedFrame& m) {
+  const DevCfg& dc = h->dc;
+  const Xform& T = m.T;
+  cudaStream_t s = m.s;
+  KSG_CUDA(cudaMemsetAsync(h->vq.counters, 0, sizeof(int) * 8, s));
+  ++h->n_launches;
+  k_voxel_heads<<<grid_for(m.n_records, kHeadsBlock), 256, 0, s>>>(dc, h->d_cnt, h->map, h->rec_b, m.n_records, h->frame_stamp, h->vq);
+  if (h->profiling) cudaEventRecord(h->ev[5], s);
+  if (h->hot_enabled) { const int rch = hot_voxel_prepass(h, s, T, m.n_records, &m.src, &m.n_hot); if (rch) return rch; }
+  const ApplySrc& src = m.src;
+  KSG_CUDA(cudaEventRecord(h->ev_fork, s));
+  KSG_CUDA(cudaStreamWaitEvent(h->aux_stream, h->ev_fork, 0));
+  // C <= 32: the voxels with thousands of records get one CTA each (third stream, concurrent with the other two kernels)
+  const int use_hot = (h->apply_nch == 1 && !h->hot_enabled && h->hot_kernel) ? 1 : 0;
+  bool deep_launched = false;
+  if (use_hot) {
+    KSG_CUDA(cudaStreamWaitEvent(h->aux_stream2, h->ev_fork, 0));
     ++h->n_launches;
-    k_block_init<<<h->sm_count * 4, 256, 0, s>>>(dc, h->d_cnt, h->map);
-    if (h->voxel_apply) {
-      // per-voxel update (ksg_voxel.cuh): segment heads -> two queues; the long and the short kernel run concurrently
-      KSG_CUDA(cudaMemsetAsync(h->vq.counters, 0, sizeof(int) * 8, s));
+    k_voxel_apply_hot<<<h->sm_count, 256, h->hot_smem, h->aux_stream2>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
+    KSG_CUDA(cudaEventRecord(h->ev_join2, h->aux_stream2));
+  }
+  h->n_launches += 2;
+  if (h->short_thread && h->apply_nch == 1) {
+    int skip = use_hot;
+    if (h->deep_hot && !use_hot) {   // the hot voxels' chains first, on their own high-priority stream (one warp per chain)
+      KSG_CUDA(cudaStreamWaitEvent(h->aux_stream2, h->ev_fork, 0));
       ++h->n_launches;
-      k_voxel_heads<<<grid_for(n_records, kHeadsBlock), 256, 0, s>>>(dc, h->d_cnt, h->map, h->rec_b, n_records, h->frame_stamp, h->vq);
-      if (h->profiling) cudaEventRecord(h->ev[5], s);
-      did_apply = true;
-      if (h->hot_enabled) {
-        int n_hot = 0;
-        const int rch = hot_voxel_prepass(h, s, T, src.param, n_records, &n_hot);
-        if (rch) return rch;
-        src.hot_segs = h->d_hot_segs; src.hot_prior = h->d_hot_prior; src.n_hot = n_hot; src.hot_thresh = kHotThresh;
-        src.hot_tsdf_same = (h->cfg.hot_voxel_mode == 2) ? h->d_hot_same : nullptr;
-        last_hot_voxels = n_hot;
-      }
-      KSG_CUDA(cudaEventRecord(h->ev_fork, s));
-      KSG_CUDA(cudaStreamWaitEvent(h->aux_stream, h->ev_fork, 0));
-      // C <= 32: the voxels with thousands of records get one CTA each (third stream, concurrent with the other two kernels)
-      const int use_hot = (h->apply_nch == 1 && !h->hot_enabled && h->hot_kernel) ? 1 : 0;
-      bool deep_launched = false;
-      if (use_hot) {
-        KSG_CUDA(cudaStreamWaitEvent(h->aux_stream2, h->ev_fork, 0));
-        ++h->n_launches;
-        k_voxel_apply_hot<<<h->sm_count, 256, h->hot_smem, h->aux_stream2>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
-        KSG_CUDA(cudaEventRecord(h->ev_join2, h->aux_stream2));
-      }
-      h->n_launches += 2;
-#define KSG_LAUNCH_VOXEL(NCH)                                                                                                             \
-      do {                                                                                                                                \
-        k_voxel_apply_long<NCH><<<h->long_grid, h->long_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, use_hot);  \
-        k_voxel_apply_short<NCH><<<h->sm_count * h->short_ctas, 256, h->short_smem, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);        \
-      } while (0)
-      if (h->short_thread && h->apply_nch == 1) {
-        int skip = use_hot;
-        if (h->deep_hot && !use_hot) {   // the hot voxels' chains first, on their own high-priority stream (one warp per chain)
-          KSG_CUDA(cudaStreamWaitEvent(h->aux_stream2, h->ev_fork, 0));
-          ++h->n_launches;
-          k_voxel_apply_long<1, true><<<h->sm_count, h->deep_threads, 0, h->aux_stream2>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, 0);
-          KSG_CUDA(cudaEventRecord(h->ev_join2, h->aux_stream2));
-          skip = 1; deep_launched = true;
-        }
-        if (h->long_serial && deep_launched) {   // the remaining long segments are little work: behind the short kernel, on its stream
-          k_voxel_apply_short_t<<<h->sm_count * h->short_t_ctas, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
-          k_voxel_apply_long<1><<<h->long_grid, h->long_threads, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, skip);
-        } else {
-          k_voxel_apply_long<1><<<h->long_grid, h->long_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, skip);
-          k_voxel_apply_short_t<<<h->sm_count * h->short_t_ctas, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
-        }
-      } else
-      switch (h->apply_nch) { case 1: KSG_LAUNCH_VOXEL(1); break; case 2: KSG_LAUNCH_VOXEL(2); break; case 4: KSG_LAUNCH_VOXEL(4); break; default: KSG_LAUNCH_VOXEL(8); break; }
-#undef KSG_LAUNCH_VOXEL
-      KSG_CUDA(cudaEventRecord(h->ev_join, h->aux_stream));
-      KSG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-      if (use_hot || deep_launched) KSG_CUDA(cudaStreamWaitEvent(s, h->ev_join2, 0));
+      k_voxel_apply_long<1, true><<<h->sm_count, h->deep_threads, 0, h->aux_stream2>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, 0);
+      KSG_CUDA(cudaEventRecord(h->ev_join2, h->aux_stream2));
+      skip = 1; deep_launched = true;
+    }
+    if (h->long_serial && deep_launched) {   // the remaining long segments are little work: behind the short kernel, on its stream
+      k_voxel_apply_short_t<<<h->sm_count * h->short_t_ctas, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
+      k_voxel_apply_long<1><<<h->long_grid, h->long_threads, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, skip);
     } else {
-    ++h->n_launches;
-    k_tile_heads<<<grid_for(n_records, B), B, 0, s>>>(dc, h->d_cnt, h->map, h->rec_b, n_records, h->frame_stamp, h->tile_begin,
+      k_voxel_apply_long<1><<<h->long_grid, h->long_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, skip);
+      k_voxel_apply_short_t<<<h->sm_count * h->short_t_ctas, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
+    }
+  } else {
+    with_nch(h->apply_nch, [&](auto nch) {
+      constexpr int NCH = decltype(nch)::value;
+      k_voxel_apply_long<NCH><<<h->long_grid, h->long_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, use_hot);
+      k_voxel_apply_short<NCH><<<h->sm_count * h->short_ctas, 256, h->short_smem, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
+    });
+  }
+  KSG_CUDA(cudaEventRecord(h->ev_join, h->aux_stream));
+  KSG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
+  if (use_hot || deep_launched) KSG_CUDA(cudaStreamWaitEvent(s, h->ev_join2, 0));
+  return KSG_OK;
+}
+
+// Tile update (apply_mode 1, KSG_MERGED_TILE_APPLY=1): one CTA walks the records of a tile
+int merged_apply_tiles(ksg_integrator* h, MergedFrame& m) {
+  const DevCfg& dc = h->dc;
+  const Xform& T = m.T;
+  cudaStream_t s = m.s;
+  const int B = 256;
+  ++h->n_launches;
+  k_tile_heads<<<grid_for(m.n_records, B), B, 0, s>>>(dc, h->d_cnt, h->map, h->rec_b, m.n_records, h->frame_stamp, h->tile_begin,
                                                       h->tile_cap);
-
-    if (h->profiling) cudaEventRecord(h->ev[5], s);
-    did_apply = true;
-    const int ctas_per_sm = std::max(1, std::min(8, (int)(220 * 1024 / std::max(1, h->apply_smem + 1024))));
-    const int grid = h->sm_count * ctas_per_sm;
-    int n_hot = 0;
-    if (h->hot_enabled) {
-      const int rch = hot_voxel_prepass(h, s, T, src.param, n_records, &n_hot);
-      if (rch) return rch;
-      src.hot_segs = h->d_hot_segs; src.hot_prior = h->d_hot_prior; src.n_hot = n_hot; src.hot_thresh = kHotThresh;
-      src.hot_tsdf_same = (h->cfg.hot_voxel_mode == 2) ? h->d_hot_same : nullptr;
-      last_hot_voxels = n_hot;
-    }
-    ++h->n_launches;
-    if (n_hot > 0) {   // C <= 32, TMA staging (checked when hot_enabled was set)
-      k_tile_apply<true, 1, true><<<grid, 256, h->apply_smem, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, n_records,
-                                                                   h->tile_begin, h->tile_cap, src, h->tile_debug);
-    } else
-#define KSG_LAUNCH_APPLY(TMA, NCH)                                                                                 \
-    k_tile_apply<TMA, NCH><<<grid, 256, h->apply_smem, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, \
-                                                            n_records, h->tile_begin, h->tile_cap, src, h->tile_debug)
-    if (h->use_tma) {
-      switch (h->apply_nch) { case 1: KSG_LAUNCH_APPLY(true, 1); break; case 2: KSG_LAUNCH_APPLY(true, 2); break;
-                              case 4: KSG_LAUNCH_APPLY(true, 4); break; default: KSG_LAUNCH_APPLY(true, 8); break; }
-    } else {
-      switch (h->apply_nch) { case 1: KSG_LAUNCH_APPLY(false, 1); break; case 2: KSG_LAUNCH_APPLY(false, 2); break;
-                              case 4: KSG_LAUNCH_APPLY(false, 4); break; default: KSG_LAUNCH_APPLY(false, 8); break; }
-    }
-#undef KSG_LAUNCH_APPLY
-    }
-    if (h->d_log_head) {
-      // update log (ksg_log.cuh), behind every apply kernel.  The unsorted record buffer (and the short queue in it) is free again:
-      // [head record indices : n_records ints][flags : n_records bytes], later [head record indices][the same, block-index order].
-      // The sort keys go to the log's own entry buffer, which the entries overwrite only after the sort (32 bytes per entry >= 16).
-      int* heads = (int*)h->rec_a;
-      int* heads_alt = heads + n_records;
-      uint8_t* flags = (uint8_t*)heads_alt;
-      ++h->n_launches;
-      k_merged_log_heads<<<grid_for(n_records, B), B, 0, s>>>(dc, h->map, h->rec_b, n_records, flags);
-      size_t tb = h->cub_temp_bytes;
-      ++h->n_libcalls;
-      KSG_CUDA(cub::DeviceSelect::Flagged(h->cub_temp, tb, cub::CountingInputIterator<int>(0), flags, heads, &h->d_cnt->pad0, (int)n_records, s));
-      int n_heads = 0;
-      KSG_CUDA(cudaMemcpyAsync(&n_heads, &h->d_cnt->pad0, sizeof(int), cudaMemcpyDeviceToHost, s));
-      KSG_CUDA(cudaStreamSynchronize(s));
-      if (n_heads > 0 && n_heads <= h->log_cap) {
-        uint64_t* keys = (uint64_t*)h->d_log_head;
-        ++h->n_launches;
-        k_merged_log_keys<<<grid_for(n_heads, B), B, 0, s>>>(dc, h->map, h->rec_b, heads, n_heads, keys);
-        cub::DoubleBuffer<uint64_t> kb(keys, keys + n_heads);
-        cub::DoubleBuffer<int> vb(heads, heads_alt);
-        tb = h->cub_temp_bytes;
-        ++h->n_libcalls;
-        KSG_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_temp, tb, kb, vb, n_heads, 0, 63, s));   // pack_key: 3 x 21 bits
-        ++h->n_launches;
-        k_merged_log_write<<<h->sm_count * 8, 256, 0, s>>>(dc, h->map, h->rec_b, vb.Current(), n_heads, h->d_log_head, h->d_log_prior);
-      }
-      log_written = true;
-    }
+  if (h->profiling) cudaEventRecord(h->ev[5], s);
+  const int ctas_per_sm = std::max(1, std::min(8, (int)(220 * 1024 / std::max(1, h->apply_smem + 1024))));
+  const int grid = h->sm_count * ctas_per_sm;
+  if (h->hot_enabled) { const int rch = hot_voxel_prepass(h, s, T, m.n_records, &m.src, &m.n_hot); if (rch) return rch; }
+  const ApplySrc& src = m.src;
+  ++h->n_launches;
+  if (m.n_hot > 0) {   // C <= 32, TMA staging (checked when hot_enabled was set)
+    k_tile_apply<true, 1, true><<<grid, 256, h->apply_smem, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, m.n_records,
+                                                                 h->tile_begin, h->tile_cap, src, h->tile_debug);
+  } else {
+    with_tma(h->use_tma, [&](auto tma) {
+      with_nch(h->apply_nch, [&](auto nch) {
+        k_tile_apply<decltype(tma)::value, decltype(nch)::value><<<grid, 256, h->apply_smem, s>>>(
+            dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, m.n_records, h->tile_begin, h->tile_cap, src, h->tile_debug);
+      });
+    });
   }
-  if (h->profiling) { if (!did_apply) { cudaEventRecord(h->ev[4], s); cudaEventRecord(h->ev[5], s); } cudaEventRecord(h->ev[6], s); }
+  return KSG_OK;
+}
+
+// Update log (ksg_log.cuh), behind every apply kernel.  The unsorted record buffer (and the short queue in it) is free again:
+// [head record indices : n_records ints][flags : n_records bytes], later [head record indices][the same, block-index order].
+// The sort keys go to the log's own entry buffer, which the entries overwrite only after the sort (32 bytes per entry >= 16).
+int merged_update_log(ksg_integrator* h, MergedFrame& m) {
+  const DevCfg& dc = h->dc;
+  cudaStream_t s = m.s;
+  const int B = 256;
+  const long long n_records = m.n_records;
+  int* heads = (int*)h->rec_a;
+  int* heads_alt = heads + n_records;
+  uint8_t* flags = (uint8_t*)heads_alt;
+  ++h->n_launches;
+  k_merged_log_heads<<<grid_for(n_records, B), B, 0, s>>>(dc, h->map, h->rec_b, n_records, flags);
+  size_t tb = h->cub_temp_bytes;
+  ++h->n_libcalls;
+  KSG_CUDA(cub::DeviceSelect::Flagged(h->cub_temp, tb, cub::CountingInputIterator<int>(0), flags, heads, &h->d_cnt->pad0, (int)n_records, s));
+  int n_heads = 0;
+  KSG_CUDA(cudaMemcpyAsync(&n_heads, &h->d_cnt->pad0, sizeof(int), cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
+  if (n_heads > 0 && n_heads <= h->log_cap) {
+    uint64_t* keys = (uint64_t*)h->d_log_head;
+    ++h->n_launches;
+    k_merged_log_keys<<<grid_for(n_heads, B), B, 0, s>>>(dc, h->map, h->rec_b, heads, n_heads, keys);
+    cub::DoubleBuffer<uint64_t> kb(keys, keys + n_heads);
+    cub::DoubleBuffer<int> vb(heads, heads_alt);
+    tb = h->cub_temp_bytes;
+    ++h->n_libcalls;
+    KSG_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_temp, tb, kb, vb, n_heads, 0, 63, s));   // pack_key: 3 x 21 bits
+    ++h->n_launches;
+    k_merged_log_write<<<h->sm_count * 8, 256, 0, s>>>(dc, h->map, h->rec_b, vb.Current(), n_heads, h->d_log_head, h->d_log_prior);
+  }
+  return KSG_OK;
+}
+
+// Completion: the frame's counters on the host, its phase times, statistics and device-side error.  `applied`: the records were
+// sorted and applied (no device-side error in the bundling, at least one record).
+int merged_complete(ksg_integrator* h, const MergedFrame& m, bool applied, ksg_frame_stats* stats) {
+  cudaStream_t s = m.s;
+  if (h->profiling) { if (!applied) { cudaEventRecord(h->ev[4], s); cudaEventRecord(h->ev[5], s); } cudaEventRecord(h->ev[6], s); }
   ++h->n_launches;
   k_frame_finish<<<1, 1, 0, s>>>(h->d_cnt, h->map);
   KSG_CUDA(cudaGetLastError());
-  rc = fetch_counters(h, s);
+  const int rc = fetch_counters(h, s);
   if (rc) return rc;
   if (h->profiling) {
     cudaEventRecord(h->ev[7], s);
@@ -862,34 +957,77 @@ int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaS
     { float ms = 0; if (cudaEventElapsedTime(&ms, h->ev[0], h->ev[7]) == cudaSuccess) h->phase_ms[6] += ms; }
     h->prof_frames += 1;
   }
-  dev_err = h->h_cnt->err;
-  h->num_blocks = h->h_cnt->pool_count;
-  h->last_blocks_touched = h->h_cnt->n_blocks_touched;
-  h->last_hot_segments = (int)last_hot_voxels;
-  if (log_written) h->merged_log_count = h->h_cnt->pad0;
-  h->last_frame_queued = did_apply && h->voxel_apply;
+  mirror_counters(h);
+  h->last_hot_segments = m.n_hot;
+  if (applied && h->d_log_head) h->merged_log_count = h->h_cnt->pad0;
+  h->last_frame_queued = applied && h->voxel_apply;
   if (stats) {
-    std::memset(stats, 0, sizeof(*stats));
-    stats->points_in = h->h_cnt->n_points;
-    stats->points_valid = h->h_cnt->n_valid;
-    stats->rays_cast = h->h_cnt->n_cast;
-    stats->ray_steps = (int64_t)h->h_cnt->ray_steps;
-    stats->voxel_updates = n_records - (int64_t)h->h_cnt->n_skipped;
-    stats->blocks_allocated = h->num_blocks;
-    stats->blocks_touched = h->h_cnt->n_blocks_touched;
-    stats->tiles_touched = h->h_cnt->n_tiles;
-    stats->hot_voxels = last_hot_voxels;
-    if (h->hot_enabled && last_hot_voxels > 0) {
+    fill_stats(h, stats);
+    stats->voxel_updates = m.n_records - (int64_t)h->h_cnt->n_skipped;   // this frame's records: none after a bundling error
+    stats->hot_voxels = m.n_hot;
+    if (h->hot_enabled && m.n_hot > 0) {
       int fb = 0;
       if (cudaMemcpyAsync(&fb, h->d_hot_counts + 1, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess && cudaStreamSynchronize(s) == cudaSuccess)
         stats->hot_fallback_chunks = fb;
     }
   }
-  if (dev_err) {
-    h->deferred_status = dev_err;  // the map may be inconsistent from here on
-    return fail(dev_err, err_text(dev_err));
+  return device_error(h);
+}
+
+// `merged` frame driver: the host reads the counters back after the bundling and at completion.
+int integrate_merged(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, const Xform& T, int cap, cudaStream_t s,
+                     ksg_frame_stats* stats) {
+  MergedFrame m{in, fin, T, cap, s};
+  h->merged_log_count = 0;
+  if (h->profiling) cudaEventRecord(h->ev[0], s);
+  { const int rc = merged_bundles(h, m); if (rc) return rc; }
+  if (h->profiling) cudaEventRecord(h->ev[2], s);
+  if (!h->h_cnt->err) merged_emit(h, m);
+  m.src.param = h->ray_param; m.src.label = nullptr; m.src.color = nullptr; m.src.tmp = h->tmp; m.src.tmp4 = h->tmp4;
+  if (h->profiling) cudaEventRecord(h->ev[3], s);
+  const bool applied = !h->h_cnt->err && m.n_records > 0;
+  if (applied) {
+    int rc = merged_sort_records(h, m);
+    if (!rc) rc = h->voxel_apply ? merged_apply_voxels(h, m) : merged_apply_tiles(h, m);
+    if (!rc && h->d_log_head) rc = merged_update_log(h, m);
+    if (rc) return rc;
   }
-  return KSG_OK;
+  return merged_complete(h, m, applied, stats);
+}
+
+int integrate(ksg_integrator* h, const InputDesc& in, const float* T_host, cudaStream_t s, ksg_frame_stats* stats) {
+  if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
+  if (in.n > h->cap_points) return h->fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");
+  if (in.n == 0 && h->n_pend > 0) { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  KSG_CUDA(cudaSetDevice(h->device));
+  const bool fast = h->cfg.integrator_type == KSG_INTEGRATOR_FAST;
+  const int cap = (int)in.n;  // host upper bound of the point count
+  Xform T{T_host[0], T_host[1], T_host[2], T_host[3], T_host[4], T_host[5], T_host[6]};
+  h->frame_stamp += 1;
+
+  if (cap == 0) {
+    if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->blocks_allocated = h->num_blocks; }
+    if (fast) { const int rcs = advance_sets(h, s); if (rcs) return rcs; }   // the sets are reset even for an empty frame
+    else h->merged_log_count = 0;
+    h->last_blocks_touched = 0;
+    return KSG_OK;
+  }
+
+  FrameIn fin{};
+  fin.xyz = in.d_xyz; fin.rgba = in.d_rgba; fin.labels = in.d_labels;
+  fin.depth = in.d_depth; fin.label_img = in.d_label_img; fin.pix_list = h->pix_list;
+  fin.point_of_seq = nullptr;
+  fin.width = in.width;
+  fin.cx = (float)in.K[2]; fin.cy = (float)in.K[3];   // depth_map_to_pointcloud.h:222-223 float center = model_.cx()
+  if (in.d_depth) {  // depth_map_to_pointcloud.h:228-230: float constant = unit_scaling / f  (double division)
+    fin.constant_x = (float)(in.unit_scaling / in.K[0]);
+    fin.constant_y = (float)(in.unit_scaling / in.K[1]);
+  }
+  fin.z_scale = in.z_scale;
+  fin.color_img = in.d_color_img;
+  fin.freespace = in.freespace;
+  if (fast) return integrate_fast(h, in, fin, T, cap, s, stats);
+  return integrate_merged(h, in, fin, T, cap, s, stats);
 }
 
 bool is_pinned_host(const void* p) {
@@ -899,19 +1037,8 @@ bool is_pinned_host(const void* p) {
 }
 
 int ensure_input(ksg_integrator* h, size_t bytes) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
-  if (bytes > h->h_stage_bytes) {
-    if (h->h_stage) cudaFreeHost(h->h_stage);
-    h->h_stage = nullptr;
-    KSG_CUDA(cudaMallocHost((void**)&h->h_stage, bytes));
-    h->h_stage_bytes = bytes;
-  }
-  if (bytes > h->d_in_bytes) {
-    if (h->d_in) cudaFree(h->d_in);
-    h->d_in = nullptr;
-    KSG_CUDA(cudaMalloc((void**)&h->d_in, bytes));
-    h->d_in_bytes = bytes;
-  }
+  if (bytes > h->h_stage_bytes) KSG_CUDA(h->res.regrow_pinned(&h->h_stage, &h->h_stage_bytes, bytes));
+  if (bytes > h->d_in_bytes) KSG_CUDA(h->res.regrow(&h->d_in, &h->d_in_bytes, bytes));
   return KSG_OK;
 }
 
@@ -979,15 +1106,17 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     cudaGetLastError();
     return KSG_ERR_NO_DEVICE;
   }
-  ksg_integrator* h = new ksg_integrator();
+  const Knobs knobs = read_knobs();
+  std::unique_ptr<ksg_integrator> owner(new ksg_integrator());   // every early return below releases what was made so far
+  ksg_integrator* h = owner.get();
+  Resources& res = h->res;
   h->cfg = *cfg;
   h->device = cfg->device;
-  auto fail = [&](int c, const char* m) { g_last_error = m; free_all(h); delete h; return c; };
   KSG_CUDA(cudaSetDevice(h->device));
   cudaDeviceProp prop;
   KSG_CUDA(cudaGetDeviceProperties(&prop, h->device));
   h->sm_count = prop.multiProcessorCount;
-  KSG_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
+  KSG_CUDA(res.stream(&h->own_stream));
 
   // ---- geometry (voxblox Layer: inverses are 1.0 / x in double, stored as float; A.1, base.cpp:84-89)
   DevCfg& dc = h->dc;
@@ -1039,166 +1168,161 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     h->h_luts.dynamic_label[l] = cfg->dynamic_label[l];
   }
   for (int i = 0; i < 1024; ++i) { h->h_luts.c2l_keys[i] = 0xFFFFFFFFu; h->h_luts.c2l_vals[i] = 0; }
-  KSG_CUDA(dmalloc(&h->d_luts, 1));
+  KSG_CUDA(res.device(&h->d_luts, 1));
   KSG_CUDA(cudaMemcpy(h->d_luts, &h->h_luts, sizeof(Luts), cudaMemcpyHostToDevice));
 
   // ---- map
   h->ht_cap = 1024;
   while (h->ht_cap < 2u * (uint32_t)cfg->max_blocks) h->ht_cap <<= 1;
-  if ((unsigned long long)h->ht_cap * dc.tiles_per_block >= (1ull << 32)) return fail(KSG_ERR_INVALID_ARGUMENT, "max_blocks too large");
+  if ((unsigned long long)h->ht_cap * dc.tiles_per_block >= (1ull << 32)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "max_blocks too large");
   h->map.ht_mask = h->ht_cap - 1;
   h->map.max_blocks = cfg->max_blocks;
   h->map.new_cap = cfg->max_blocks;
-  KSG_CUDA(dmalloc(&h->map.ht_keys, h->ht_cap));
-  KSG_CUDA(dmalloc(&h->map.ht_slot, h->ht_cap));
-  KSG_CUDA(dmalloc(&h->map.touched_stamp, h->ht_cap));
-  KSG_CUDA(dmalloc(&h->map.touched_list, h->ht_cap));
-  KSG_CUDA(dmalloc(&h->map.new_list, (size_t)cfg->max_blocks));
-  KSG_CUDA(dmalloc(&h->map.slot_key, (size_t)cfg->max_blocks));
-  KSG_CUDA(cudaMalloc((void**)&h->map.pool, (size_t)dc.block_stride * (size_t)cfg->max_blocks));
-  KSG_CUDA(dmalloc(&h->d_cnt, 1));
-  KSG_CUDA(cudaMallocHost((void**)&h->h_cnt_base, 2 * sizeof(Counters)));
+  KSG_CUDA(res.device(&h->map.ht_keys, h->ht_cap));
+  KSG_CUDA(res.device(&h->map.ht_slot, h->ht_cap));
+  KSG_CUDA(res.device(&h->map.touched_stamp, h->ht_cap));
+  KSG_CUDA(res.device(&h->map.touched_list, h->ht_cap));
+  KSG_CUDA(res.device(&h->map.new_list, (size_t)cfg->max_blocks));
+  KSG_CUDA(res.device(&h->map.slot_key, (size_t)cfg->max_blocks));
+  KSG_CUDA(res.device(&h->map.pool, (size_t)dc.block_stride * (size_t)cfg->max_blocks));
+  KSG_CUDA(res.device(&h->d_cnt, 1));
+  KSG_CUDA(res.pinned(&h->h_cnt_base, 2));
   std::memset(h->h_cnt_base, 0, 2 * sizeof(Counters));
   h->h_cnt = h->h_cnt_base;
   for (int i = 0; i < 2; ++i) {
-    KSG_CUDA(cudaEventCreateWithFlags(&h->ev_frame_s[i], cudaEventDisableTiming));
-    KSG_CUDA(cudaEventCreateWithFlags(&h->ev_copy[i], cudaEventDisableTiming));
-    KSG_CUDA(cudaEventCreateWithFlags(&h->ev_free[i], cudaEventDisableTiming));
+    KSG_CUDA(res.event(&h->ev_frame_s[i], cudaEventDisableTiming));
+    KSG_CUDA(res.event(&h->ev_copy[i], cudaEventDisableTiming));
+    KSG_CUDA(res.event(&h->ev_free[i], cudaEventDisableTiming));
   }
-  KSG_CUDA(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+  KSG_CUDA(res.stream(&h->copy_stream));
 
   // ---- frame scratch
   const size_t N = (size_t)cfg->max_points;
   h->cap_points = cfg->max_points;
   const bool fast = cfg->integrator_type == KSG_INTEGRATOR_FAST;
-  KSG_CUDA(dmalloc(&h->pt_pC, N)); KSG_CUDA(dmalloc(&h->pt_pG, N));
-  KSG_CUDA(dmalloc(&h->pt_label, N)); KSG_CUDA(dmalloc(&h->pt_flags, N));
-  KSG_CUDA(dmalloc(&h->pt_color, N)); KSG_CUDA(dmalloc(&h->pt_key, N));
-  KSG_CUDA(dmalloc(&h->flags8, 2 * N));
-  KSG_CUDA(dmalloc(&h->pix_list, N));
-  KSG_CUDA(dmalloc(&h->iota, N));
+  KSG_CUDA(res.device(&h->pt_pC, N)); KSG_CUDA(res.device(&h->pt_pG, N));
+  KSG_CUDA(res.device(&h->pt_label, N)); KSG_CUDA(res.device(&h->pt_flags, N));
+  KSG_CUDA(res.device(&h->pt_color, N)); KSG_CUDA(res.device(&h->pt_key, N));
+  KSG_CUDA(res.device(&h->flags8, 2 * N));
+  KSG_CUDA(res.device(&h->pix_list, N));
+  KSG_CUDA(res.device(&h->iota, N));
   k_iota<<<grid_for((long long)N, 256), 256>>>(h->iota, (int)N);
   if (cfg->integration_order_mode == KSG_ORDER_SORTED) {
-    KSG_CUDA(dmalloc(&h->point_of_seq, N)); KSG_CUDA(dmalloc(&h->sq_keys, N)); KSG_CUDA(dmalloc(&h->sq_keys_out, N));
+    KSG_CUDA(res.device(&h->point_of_seq, N)); KSG_CUDA(res.device(&h->sq_keys, N)); KSG_CUDA(res.device(&h->sq_keys_out, N));
   }
-  KSG_CUDA(dmalloc(&h->ray_param, N)); KSG_CUDA(dmalloc(&h->ray_flags, N)); KSG_CUDA(dmalloc(&h->nsteps, N));
+  KSG_CUDA(res.device(&h->ray_param, N)); KSG_CUDA(res.device(&h->ray_flags, N)); KSG_CUDA(res.device(&h->nsteps, N));
   long long rec_cap = cfg->max_updates > 0 ? cfg->max_updates : (fast ? std::max<long long>(4ll << 20, 64ll * (long long)N) : (64ll << 20));
   if (fast) {
-    KSG_CUDA(dmalloc(&h->start_next, N)); KSG_CUDA(dmalloc(&h->start_table, kSetSize));
+    KSG_CUDA(res.device(&h->start_next, N)); KSG_CUDA(res.device(&h->start_table, kSetSize));
     // per-frame cleared arrays live in two contiguous regions, so that a frame needs three memsets instead of seven:
     //   0xFF: [s_base | start_max | s_hmin | o3.head]               4 + 4 + 4 + 4 bytes per slot
     //   0x00: [o3.slot_cnt | (unused) | s_hmax | s_visits]          4 + 1 + 4 + 4 bytes per slot
-    KSG_CUDA(cudaMalloc((void**)&h->clear_ff, (size_t)kSetSize * 16));
-    KSG_CUDA(cudaMalloc((void**)&h->clear_00, (size_t)kSetSize * 13));
+    KSG_CUDA(res.device(&h->clear_ff, (size_t)kSetSize * 16));
+    KSG_CUDA(res.device(&h->clear_00, (size_t)kSetSize * 13));
     h->s_base = (int*)h->clear_ff; h->start_max = h->s_base + kSetSize; h->s_hmin = (uint32_t*)(h->start_max + kSetSize);
     h->o3.head = (int*)(h->clear_ff + (size_t)kSetSize * 12);
     h->o3.slot_cnt = (int*)h->clear_00;
     h->s_hmax = (uint32_t*)(h->clear_00 + (size_t)kSetSize * 5); h->s_visits = (int*)(h->clear_00 + (size_t)kSetSize * 9);
-    KSG_CUDA(dmalloc(&h->start_min, kSetSize));
-    KSG_CUDA(dmalloc(&h->cast_seq, N));
-    KSG_CUDA(dmalloc(&h->ray_label, N)); KSG_CUDA(dmalloc(&h->ray_color, N));
-    KSG_CUDA(dmalloc(&h->ray_state, N)); KSG_CUDA(dmalloc(&h->ext_off, N * kExtSegs));
+    KSG_CUDA(res.device(&h->start_min, kSetSize));
+    KSG_CUDA(res.device(&h->cast_seq, N));
+    KSG_CUDA(res.device(&h->ray_label, N)); KSG_CUDA(res.device(&h->ray_color, N));
+    KSG_CUDA(res.device(&h->ray_state, N)); KSG_CUDA(res.device(&h->ext_off, N * kExtSegs));
     long long ext = cfg->max_ray_steps > 0 ? cfg->max_ray_steps : std::max<long long>(16ll << 20, 64ll * (long long)N);
     Obs3& o3 = h->o3;
     o3.ext_base = (long long)N * kH0;
     o3.cand_cap = o3.ext_base + ext;
     if (o3.cand_cap >= 0x7FFFFFFFll) { o3.cand_cap = 0x7FFFFFFEll; }
-    KSG_CUDA(cudaMalloc((void**)&o3.cand, sizeof(Cand) * (size_t)o3.cand_cap));
+    KSG_CUDA(res.device(&o3.cand, (size_t)o3.cand_cap));
     o3.ovf_cap = (int)std::min<long long>(std::max<long long>(1ll << 20, 4ll * (long long)N), 1ll << 28);
-    KSG_CUDA(cudaMalloc((void**)&o3.ovf, sizeof(OvfEnt) * (size_t)o3.ovf_cap));
-    KSG_CUDA(dmalloc(&o3.bkt, (size_t)kSetSize * kBkt3));
-    KSG_CUDA(dmalloc(&o3.stamp_max, 2 * (size_t)kSetSize)); o3.stamp_min = o3.stamp_max + kSetSize;
-    KSG_CUDA(dmalloc(&o3.table, kSetSize));
-    KSG_CUDA(cudaMalloc((void**)&h->rayrec, sizeof(RayRec) * N));
-    KSG_CUDA(dmalloc(&h->wl, 3 * N));
-    KSG_CUDA(dmalloc(&h->mixed_list, N)); KSG_CUDA(dmalloc(&h->m_list, N));
-    KSG_CUDA(dmalloc(&h->blk_run, (size_t)(o3.cand_cap / 16 + 16)));
+    KSG_CUDA(res.device(&o3.ovf, (size_t)o3.ovf_cap));
+    KSG_CUDA(res.device(&o3.bkt, (size_t)kSetSize * kBkt3));
+    KSG_CUDA(res.device(&o3.stamp_max, 2 * (size_t)kSetSize)); o3.stamp_min = o3.stamp_max + kSetSize;
+    KSG_CUDA(res.device(&o3.table, kSetSize));
+    KSG_CUDA(res.device(&h->rayrec, N));
+    KSG_CUDA(res.device(&h->wl, 3 * N));
+    KSG_CUDA(res.device(&h->mixed_list, N)); KSG_CUDA(res.device(&h->m_list, N));
+    KSG_CUDA(res.device(&h->blk_run, (size_t)(o3.cand_cap / 16 + 16)));
   } else {
-    KSG_CUDA(dmalloc(&h->ks_sorted, N)); KSG_CUDA(dmalloc(&h->seq_sorted, N));
-    KSG_CUDA(dmalloc(&h->bstart, 2 * N)); KSG_CUDA(dmalloc(&h->bundle_f, N));
-    KSG_CUDA(dmalloc(&h->hist, N * dc.C)); KSG_CUDA(dmalloc(&h->tmp, (N + 1) * dc.C));  // + the all-zero row
-    KSG_CUDA(dmalloc(&h->b_key, N)); KSG_CUDA(dmalloc(&h->b_base, N));
-    KSG_CUDA(dmalloc(&h->d_scan_tot, 16));
+    KSG_CUDA(res.device(&h->ks_sorted, N)); KSG_CUDA(res.device(&h->seq_sorted, N));
+    KSG_CUDA(res.device(&h->bstart, 2 * N)); KSG_CUDA(res.device(&h->bundle_f, N));
+    KSG_CUDA(res.device(&h->hist, N * dc.C)); KSG_CUDA(res.device(&h->tmp, (N + 1) * dc.C));  // + the all-zero row
+    KSG_CUDA(res.device(&h->b_key, N)); KSG_CUDA(res.device(&h->b_base, N));
+    KSG_CUDA(res.device(&h->d_scan_tot, 16));
     // per-voxel apply kernels (default); the tile kernel stays for apply_mode 1 and KSG_MERGED_TILE_APPLY=1
-    h->voxel_apply = cfg->apply_mode == 0;
-    if (const char* e = std::getenv("KSG_MERGED_TILE_APPLY")) if (std::atoi(e) != 0) h->voxel_apply = false;
+    h->voxel_apply = cfg->apply_mode == 0 && !knobs.tile_apply;
     if (h->voxel_apply) {
       h->vq.long_cap = 4 * (rec_cap / kLongLen) + 64;
       h->vq.long_len = kLongLen;
-      if (dc.C <= 32) {   // one thread per short voxel (ksg_voxel.cuh); KSG_SHORT_THREAD=0 selects the warp-per-voxel kernel, KSG_LONG_LEN the split
-        h->short_thread = true;
-        if (const char* e = std::getenv("KSG_SHORT_THREAD")) h->short_thread = std::atoi(e) != 0;
+      if (dc.C <= 32) {   // one thread per short voxel (ksg_voxel.cuh), unless KSG_SHORT_THREAD=0 selects the warp-per-voxel kernel
+        h->short_thread = knobs.short_thread;
         if (h->short_thread) {
-          KSG_CUDA(dmalloc(&h->tmp4, (N + 1) * (size_t)((dc.C + 3) & ~3)));
-          h->vq.long_len = kLongLenThread;
-          if (const char* e = std::getenv("KSG_LONG_LEN")) h->vq.long_len = std::max(kLongLen, std::min(1 << 20, std::atoi(e)));
+          KSG_CUDA(res.device(&h->tmp4, (N + 1) * (size_t)((dc.C + 3) & ~3)));
+          h->vq.long_len = knobs.long_len ? knobs.long_len : kLongLenThread;
         }
       }
       h->vq.short_cap = rec_cap;
-      KSG_CUDA(dmalloc(&h->vq.long_items, (size_t)h->vq.long_cap));
-      KSG_CUDA(dmalloc(&h->vq.counters, 8));
+      KSG_CUDA(res.device(&h->vq.long_items, (size_t)h->vq.long_cap));
+      KSG_CUDA(res.device(&h->vq.counters, 8));
       {   // the long-segment kernel must get its CTAs placed before the short-segment kernel fills the register files: its stream has priority
         int lo_p = 0, hi_p = 0;
         KSG_CUDA(cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
-        KSG_CUDA(cudaStreamCreateWithPriority(&h->aux_stream, cudaStreamNonBlocking, hi_p));
+        KSG_CUDA(res.stream(&h->aux_stream, hi_p));
       }
-      KSG_CUDA(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-      KSG_CUDA(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
+      KSG_CUDA(res.event(&h->ev_fork, cudaEventDisableTiming));
+      KSG_CUDA(res.event(&h->ev_join, cudaEventDisableTiming));
       {
         int lo_p = 0, hi_p = 0;
         KSG_CUDA(cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
-        KSG_CUDA(cudaStreamCreateWithPriority(&h->aux_stream2, cudaStreamNonBlocking, hi_p));
+        KSG_CUDA(res.stream(&h->aux_stream2, hi_p));
       }
-      KSG_CUDA(cudaEventCreateWithFlags(&h->ev_join2, cudaEventDisableTiming));
-      if (const char* e = std::getenv("KSG_L2_PERSIST")) {
+      KSG_CUDA(res.event(&h->ev_join2, cudaEventDisableTiming));
+      if (knobs.l2_persist) {
         // experiment: keep the (L * freq) rows resident in L2 while the update kernels stream records and voxel data through it
-        if (std::atoi(e) != 0) {
-          cudaDeviceProp prop{};
-          KSG_CUDA(cudaGetDeviceProperties(&prop, h->device));
-          const size_t want = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, 32u << 20);
-          if (want > 0) {
-            KSG_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want));
-            cudaStreamAttrValue attr{};
-            attr.accessPolicyWindow.base_ptr = h->tmp;
-            attr.accessPolicyWindow.num_bytes = std::min<size_t>((size_t)(N + 1) * dc.C * sizeof(float), (size_t)prop.accessPolicyMaxWindowSize);
-            attr.accessPolicyWindow.hitRatio = 1.0f;
-            attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-            attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-            KSG_CUDA(cudaStreamSetAttribute(h->aux_stream2, cudaStreamAttributeAccessPolicyWindow, &attr));
-            KSG_CUDA(cudaStreamSetAttribute(h->aux_stream, cudaStreamAttributeAccessPolicyWindow, &attr));
-          }
+        cudaDeviceProp prop{};
+        KSG_CUDA(cudaGetDeviceProperties(&prop, h->device));
+        const size_t want = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, 32u << 20);
+        if (want > 0) {
+          KSG_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want));
+          cudaStreamAttrValue attr{};
+          attr.accessPolicyWindow.base_ptr = h->tmp;
+          attr.accessPolicyWindow.num_bytes = std::min<size_t>((size_t)(N + 1) * dc.C * sizeof(float), (size_t)prop.accessPolicyMaxWindowSize);
+          attr.accessPolicyWindow.hitRatio = 1.0f;
+          attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+          attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
+          KSG_CUDA(cudaStreamSetAttribute(h->aux_stream2, cudaStreamAttributeAccessPolicyWindow, &attr));
+          KSG_CUDA(cudaStreamSetAttribute(h->aux_stream, cudaStreamAttributeAccessPolicyWindow, &attr));
         }
       }
       h->hot_smem = 2 * kHotChunkRecs * (32 * (int)sizeof(float) + (int)sizeof(float4));
       KSG_CUDA(cudaFuncSetAttribute(k_voxel_apply_hot, cudaFuncAttributeMaxDynamicSharedMemorySize, h->hot_smem));
-      if (const char* e = std::getenv("KSG_HOT_KERNEL")) h->hot_kernel = std::atoi(e) != 0;
-      h->long_grid = h->sm_count;
-      if (const char* e = std::getenv("KSG_LONG_THREADS")) { const int t = std::atoi(e); if (t == 64 || t == 128 || t == 256) h->long_threads = t; }
-      if (const char* e = std::getenv("KSG_LONG_GRID")) h->long_grid = std::max(1, std::atoi(e));
-      if (const char* e = std::getenv("KSG_DEEP_HOT")) h->deep_hot = std::atoi(e) != 0;
-      if (const char* e = std::getenv("KSG_LONG_SERIAL")) h->long_serial = std::atoi(e) != 0;
-      if (const char* e = std::getenv("KSG_DEEP_THREADS")) { const int t = std::atoi(e); if (t == 32 || t == 64 || t == 128 || t == 256) h->deep_threads = t; }
-      if (const char* e = std::getenv("KSG_SHORT_T_CTAS")) h->short_t_ctas = std::max(1, std::min(8, std::atoi(e)));
-      if (const char* e = std::getenv("KSG_SHORT_CTAS")) h->short_ctas = std::max(1, std::min(6, std::atoi(e)));
+      h->hot_kernel = knobs.hot_kernel;
+      h->long_threads = knobs.long_threads;
+      h->long_grid = knobs.long_grid ? knobs.long_grid : h->sm_count;
+      h->deep_hot = knobs.deep_hot;
+      h->long_serial = knobs.long_serial;
+      h->deep_threads = knobs.deep_threads;
+      h->short_t_ctas = knobs.short_t_ctas;
+      h->short_ctas = knobs.short_ctas;
       if (h->short_ctas < 6) {
         h->short_smem = std::min(200 * 1024, (220 * 1024) / h->short_ctas - 2048);
-        KSG_CUDA(cudaFuncSetAttribute(k_voxel_apply_short<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->short_smem));
-        KSG_CUDA(cudaFuncSetAttribute(k_voxel_apply_short<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->short_smem));
-        KSG_CUDA(cudaFuncSetAttribute(k_voxel_apply_short<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->short_smem));
-        KSG_CUDA(cudaFuncSetAttribute(k_voxel_apply_short<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->short_smem));
+        rc = for_each_nch([&](auto nch) -> int {
+          KSG_CUDA(cudaFuncSetAttribute(k_voxel_apply_short<decltype(nch)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->short_smem));
+          return KSG_OK;
+        });
+        if (rc) return rc;
       }
-      if (const char* e = std::getenv("KSG_EMIT_WARP")) h->emit_warp = std::atoi(e) != 0;
+      h->emit_warp = knobs.emit_warp;
     }
     if (cfg->hot_voxel_mode >= 1 && dc.C <= 32 && cfg->apply_mode == 0) {
       h->hot_enabled = true;
       h->hot_chunk_cap = rec_cap / kHotChunk + kHotMaxSegs;
-      KSG_CUDA(dmalloc(&h->d_hot_segs, kHotMaxSegs)); KSG_CUDA(dmalloc(&h->d_hot_counts, 2));
+      KSG_CUDA(res.device(&h->d_hot_segs, kHotMaxSegs)); KSG_CUDA(res.device(&h->d_hot_counts, 2));
       KSG_CUDA(cudaMemset(h->d_hot_counts, 0, 2 * sizeof(int)));
-      KSG_CUDA(cudaMallocHost((void**)&h->h_hot_segs, sizeof(HotSeg) * kHotMaxSegs));
-      KSG_CUDA(cudaMallocHost((void**)&h->h_hot_chunk_seg, sizeof(int) * (size_t)h->hot_chunk_cap));
-      KSG_CUDA(dmalloc(&h->d_hot_chunk_seg, (size_t)h->hot_chunk_cap)); KSG_CUDA(dmalloc(&h->d_hot_guess, (size_t)h->hot_chunk_cap * 32));
-      KSG_CUDA(dmalloc(&h->d_hot_sums, (size_t)h->hot_chunk_cap * 32)); KSG_CUDA(dmalloc(&h->d_hot_tables, (size_t)h->hot_chunk_cap * 32));
-      KSG_CUDA(dmalloc(&h->d_hot_prior, (size_t)kHotMaxSegs * 32)); KSG_CUDA(dmalloc(&h->d_hot_same, (size_t)kHotMaxSegs));
+      KSG_CUDA(res.pinned(&h->h_hot_segs, kHotMaxSegs));
+      KSG_CUDA(res.pinned(&h->h_hot_chunk_seg, (size_t)h->hot_chunk_cap));
+      KSG_CUDA(res.device(&h->d_hot_chunk_seg, (size_t)h->hot_chunk_cap)); KSG_CUDA(res.device(&h->d_hot_guess, (size_t)h->hot_chunk_cap * 32));
+      KSG_CUDA(res.device(&h->d_hot_sums, (size_t)h->hot_chunk_cap * 32)); KSG_CUDA(res.device(&h->d_hot_tables, (size_t)h->hot_chunk_cap * 32));
+      KSG_CUDA(res.device(&h->d_hot_prior, (size_t)kHotMaxSegs * 32)); KSG_CUDA(res.device(&h->d_hot_same, (size_t)kHotMaxSegs));
       KSG_CUDA(cudaFuncSetAttribute(k_hot_chunk_tables, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * 32 * kHotColStride)));
     }
     if (cfg->merged_bundle_order == KSG_BUNDLE_ORDER_LIBSTDCXX) {
@@ -1209,12 +1333,12 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
         probe.emplace((uint64_t)i, 0);
         if (probe.bucket_count() != last) { last = probe.bucket_count(); h->bord_phases.push_back(std::make_pair((int)i, (uint32_t)last)); }
       }
-      if (last >= 0x7fffffffull) return fail(KSG_ERR_INVALID_ARGUMENT, "max_points too large for merged_bundle_order");
-      KSG_CUDA(dmalloc(&h->bord_hash, N)); KSG_CUDA(dmalloc(&h->bundle_f2, N));
+      if (last >= 0x7fffffffull) return h->fail(KSG_ERR_INVALID_ARGUMENT, "max_points too large for merged_bundle_order");
+      KSG_CUDA(res.device(&h->bord_hash, N)); KSG_CUDA(res.device(&h->bundle_f2, N));
       {   // scratch of k_bundle_order: [ord_a | ord_b | next | size_at | rank : N each][first | head : 2 * last each][cta_tot][phase tables]
         const size_t np = h->bord_phases.size();
         const size_t ints = 5 * N + 4 * last + 2 * kBordCluster + 2 * np + 64;
-        KSG_CUDA(dmalloc(&h->bord_scratch, ints));
+        KSG_CUDA(res.device(&h->bord_scratch, ints));
         int* p = h->bord_scratch;
         BordBuf& bb = h->bord;
         bb.hash = h->bord_hash;
@@ -1230,10 +1354,10 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     }
   }
   h->rec_cap = rec_cap;
-  KSG_CUDA(dmalloc(&h->rec_a, (size_t)rec_cap)); KSG_CUDA(dmalloc(&h->rec_b, (size_t)rec_cap));
+  KSG_CUDA(res.device(&h->rec_a, (size_t)rec_cap)); KSG_CUDA(res.device(&h->rec_b, (size_t)rec_cap));
   h->vq.short_items = (unsigned long long*)h->rec_a;   // the unsorted record buffer is free once the sort has run
   h->tile_cap = (long long)std::min<unsigned long long>((unsigned long long)cfg->max_blocks * dc.tiles_per_block, (unsigned long long)rec_cap);
-  KSG_CUDA(dmalloc(&h->tile_begin, (size_t)h->tile_cap));
+  KSG_CUDA(res.device(&h->tile_begin, (size_t)h->tile_cap));
 
   // ---- CUB temp storage: the largest of every call made per frame
   {
@@ -1243,8 +1367,7 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     cub::DeviceRadixSort::SortPairs(nullptr, t, h->iota, h->iota, h->iota, h->iota, (int)N, 0, 32); need = std::max(need, t);
     cub::DeviceSelect::Flagged(nullptr, t, cub::CountingInputIterator<int>(0), h->flags8, h->pix_list, (int*)nullptr, (int)(2 * N));
     need = std::max(need, t);
-    h->cub_temp_bytes = need + 256;
-    KSG_CUDA(cudaMalloc(&h->cub_temp, h->cub_temp_bytes));
+    KSG_CUDA(res.regrow(&h->cub_temp, &h->cub_temp_bytes, need + 256));
   }
 
   // ---- tile-apply launch configuration
@@ -1254,72 +1377,67 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     h->apply_smem = (int)(stage + (size_t)V * 8 + 64);
     h->apply_nch = dc.C <= 32 ? 1 : (dc.C <= 64 ? 2 : (dc.C <= 128 ? 4 : 8));
     h->use_tma = cfg->apply_mode == 0;
-#define KSG_ATTR(TMA, NCH) \
-    KSG_CUDA(cudaFuncSetAttribute(k_tile_apply<TMA, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->apply_smem))
     KSG_CUDA(cudaFuncSetAttribute(k_tile_apply<true, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->apply_smem));
-    KSG_ATTR(true, 1); KSG_ATTR(true, 2); KSG_ATTR(true, 4); KSG_ATTR(true, 8);
-    KSG_ATTR(false, 1); KSG_ATTR(false, 2); KSG_ATTR(false, 4); KSG_ATTR(false, 8);
-#undef KSG_ATTR
+    rc = for_each_tma_nch([&](auto tma, auto nch) -> int {
+      KSG_CUDA(cudaFuncSetAttribute(k_tile_apply<decltype(tma)::value, decltype(nch)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    h->apply_smem));
+      return KSG_OK;
+    });
+    if (rc) return rc;
   }
   if (fast) {
     // frame driver (ksg_fast.cuh)
-    KSG_CUDA(dmalloc(&h->d_fc, 1));
+    KSG_CUDA(res.device(&h->d_fc, 1));
     KSG_CUDA(cudaMemset(h->d_fc, 0, sizeof(FastCounters)));
-    KSG_CUDA(cudaMallocHost((void**)&h->h_fc_base, 2 * sizeof(FastCounters)));
+    KSG_CUDA(res.pinned(&h->h_fc_base, 2));
     std::memset(h->h_fc_base, 0, 2 * sizeof(FastCounters));
     h->h_fc = h->h_fc_base;
-    KSG_CUDA(dmalloc(&h->blk_cnt, N / kCountBlock + 2)); KSG_CUDA(dmalloc(&h->blk_off, N / kCountBlock + 2));
-    KSG_CUDA(dmalloc(&h->warp_cnt, N / 32 + 64)); KSG_CUDA(dmalloc(&h->warp_off, N / 32 + 64));
-    if (cfg->integration_order_mode == KSG_ORDER_SORTED) KSG_CUDA(dmalloc(&h->seq_of_i, N));
-    KSG_CUDA(dmalloc(&h->keys32, (size_t)rec_cap));
+    KSG_CUDA(res.device(&h->blk_cnt, N / kCountBlock + 2)); KSG_CUDA(res.device(&h->blk_off, N / kCountBlock + 2));
+    KSG_CUDA(res.device(&h->warp_cnt, N / 32 + 64)); KSG_CUDA(res.device(&h->warp_off, N / 32 + 64));
+    if (cfg->integration_order_mode == KSG_ORDER_SORTED) KSG_CUDA(res.device(&h->seq_of_i, N));
+    KSG_CUDA(res.device(&h->keys32, (size_t)rec_cap));
     const size_t n_tk = (size_t)h->ht_cap * dc.tiles_per_block;
-    KSG_CUDA(dmalloc(&h->tile_cnt, n_tk)); KSG_CUDA(dmalloc(&h->tile_slot, n_tk));
+    KSG_CUDA(res.device(&h->tile_cnt, n_tk)); KSG_CUDA(res.device(&h->tile_slot, n_tk));
     KSG_CUDA(cudaMemset(h->tile_cnt, 0, sizeof(int) * n_tk));
-    KSG_CUDA(dmalloc(&h->tile_list, (size_t)h->tile_cap));
+    KSG_CUDA(res.device(&h->tile_list, (size_t)h->tile_cap));
     {
       int per_sm = 0;
-      if (const char* e = std::getenv("KSG_SOLVE_THREADS")) { const int t = std::atoi(e); if (t == 256 || t == 512 || t == 1024) h->solve_threads = t; }
+      h->solve_threads = knobs.solve_threads;
       h->solve_smem = (int)(sizeof(int) * kSortPerWarp * (h->solve_threads / 32));
       KSG_CUDA(cudaFuncSetAttribute(k_fast_solve3, cudaFuncAttributeMaxDynamicSharedMemorySize, h->solve_smem));
       KSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fast_solve3, h->solve_threads, (size_t)h->solve_smem));
       int coop = 0;
       cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, h->device);
       // k_fast_solve3 is a cooperative launch with every CTA resident (grid barriers between its phases)
-      if (!coop || per_sm <= 0) return fail(KSG_ERR_NO_DEVICE, "this device cannot run the fast integrator's observed-set solver "
-                                                                "(k_fast_solve3 needs a cooperative launch with at least one CTA per SM)");
-      h->solve_grid = h->sm_count * std::max(1, per_sm);
-      if (const char* e = std::getenv("KSG_SOLVE_CTAS_PER_SM")) h->solve_grid = h->sm_count * std::max(1, std::min(per_sm, std::atoi(e)));
-      if (const char* e = std::getenv("KSG_PROFILE_MARKS_ONLY")) h->profile_marks_only = std::atoi(e) != 0;
+      if (!coop || per_sm <= 0) return h->fail(KSG_ERR_NO_DEVICE, "this device cannot run the fast integrator's observed-set solver "
+                                                                   "(k_fast_solve3 needs a cooperative launch with at least one CTA per SM)");
+      h->solve_grid = h->sm_count * std::max(1, std::min(per_sm, knobs.solve_ctas_per_sm));
+      h->profile_marks_only = knobs.profile_marks_only;
       int khz = 0;
       if (cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, h->device) == cudaSuccess && khz > 0) h->clock_khz = khz;
     }
     {
       const size_t stage = dc.head_bytes + (dc.full_stage ? dc.prior_bytes : 0u);
       h->apply_fast_smem = (int)(stage + (size_t)dc.tile_voxels * 10 + 16 + 2 * sizeof(uint32_t) * kFastKeyCap + 64 + 32 + (size_t)kFastPref * 21);
-#define KSG_ATTRF(TMA, NCH) KSG_CUDA(cudaFuncSetAttribute(k_tile_apply_fast<TMA, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->apply_fast_smem))
-      KSG_ATTRF(true, 1); KSG_ATTRF(true, 2); KSG_ATTRF(true, 4); KSG_ATTRF(true, 8);
-      KSG_ATTRF(false, 1); KSG_ATTRF(false, 2); KSG_ATTRF(false, 4); KSG_ATTRF(false, 8);
-#undef KSG_ATTRF
+      rc = for_each_tma_nch([&](auto tma, auto nch) -> int {
+        KSG_CUDA(cudaFuncSetAttribute(k_tile_apply_fast<decltype(tma)::value, decltype(nch)::value>,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, h->apply_fast_smem));
+        return KSG_OK;
+      });
+      if (rc) return rc;
     }
   }
   KSG_CUDA(cudaDeviceSynchronize());
-  {
-    int r2 = reset_map(h, h->own_stream);
-    if (r2) { std::string m = h->err; return fail(r2, m.c_str()); }
-  }
-  *out = h;
+  rc = reset_map(h, h->own_stream);
+  if (rc) return rc;
+  *out = owner.release();
   return KSG_OK;
 }
 
-void ksg_destroy(ksg_integrator* h) {
-  if (!h) return;
-  free_all(h);
-  delete h;
-}
+void ksg_destroy(ksg_integrator* h) { delete h; }
 
 int32_t ksg_set_color_to_label(ksg_integrator* h, const uint8_t* rgb, const uint8_t* labels, int32_t n) {
   if (!h || n < 0 || n > 512 || (n > 0 && (!rgb || !labels))) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   for (int i = 0; i < 1024; ++i) { h->h_luts.c2l_keys[i] = 0xFFFFFFFFu; h->h_luts.c2l_vals[i] = 0; }
   for (int i = 0; i < n; ++i) {
     const uint32_t key = (uint32_t)rgb[3 * i] | ((uint32_t)rgb[3 * i + 1] << 8) | ((uint32_t)rgb[3 * i + 2] << 16);
@@ -1360,10 +1478,9 @@ int32_t ksg_integrate_depth_device(ksg_integrator* h, const float* T, const floa
 int32_t ksg_integrate_points(ksg_integrator* h, const float* T, const float* xyz, const uint8_t* rgba, const uint8_t* labels,
                              int64_t n, int32_t freespace, ksg_frame_stats* stats) {
   if (!h || !T || n < 0 || (n > 0 && !xyz)) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
-  if (n > h->cap_points) return fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");   // before any staging copy
+  if (n > h->cap_points) return h->fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");   // before any staging copy
   if (h->cfg.integrator_type == KSG_INTEGRATOR_MERGED && rgba && labels && h->cfg.color_mode == KSG_COLOR_MODE_COLOR)
-    return fail(KSG_ERR_INVALID_ARGUMENT, "merged, ColorMode::kColor: explicit labels together with point colours are not supported (see ksg.h)");
+    return h->fail(KSG_ERR_INVALID_ARGUMENT, "merged, ColorMode::kColor: explicit labels together with point colours are not supported (see ksg.h)");
   KSG_CUDA(cudaSetDevice(h->device));
   auto up256 = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t b_xyz = (size_t)n * 12, b_rgba = rgba ? (size_t)n * 4 : 0, b_lab = labels ? (size_t)n : 0;
@@ -1386,10 +1503,9 @@ int32_t ksg_integrate_points(ksg_integrator* h, const float* T, const float* xyz
 int32_t ksg_integrate_depth_k64(ksg_integrator* h, const float* T, const float* depth, const uint8_t* label, int32_t width,
                                 int32_t height, const double* K, ksg_frame_stats* stats) {
   if (!h || !T || !K || width <= 0 || height <= 0 || !depth || !label) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   const size_t P = (size_t)width * height;
-  if ((int64_t)P > h->cap_points) return fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");   // before any staging copy
+  if ((int64_t)P > h->cap_points) return h->fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");   // before any staging copy
   const size_t o_lab = (P * 4 + 255) / 256 * 256;
   const size_t total = o_lab + (P + 255) / 256 * 256;
   int rc = ensure_input(h, total);
@@ -1431,10 +1547,9 @@ int32_t ksg_integrate_image(ksg_integrator* h, const float* T, const void* depth
   if (!h || !T || !K || width <= 0 || height <= 0 || !depth || !semantic) return KSG_ERR_INVALID_ARGUMENT;
   if (depth_type != KSG_DEPTH_F32_METRES && depth_type != KSG_DEPTH_U16_MILLIMETRES) return KSG_ERR_INVALID_ARGUMENT;
   if (semantic_type != KSG_SEMANTIC_LABEL_U8 && semantic_type != KSG_SEMANTIC_RGB8) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   const size_t P = (size_t)width * height;
-  if ((int64_t)P > h->cap_points) return fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");
+  if ((int64_t)P > h->cap_points) return h->fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");
   auto up = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t b_depth = P * (depth_type == KSG_DEPTH_U16_MILLIMETRES ? 2 : 4), b_sem = P * (semantic_type == KSG_SEMANTIC_RGB8 ? 3 : 1);
   // device staging: [raw depth | raw semantic | float depth | label | colour]
@@ -1477,22 +1592,19 @@ int32_t ksg_integrate_depth(ksg_integrator* h, const float* T, const float* dept
 int32_t ksg_integrate_depth_async(ksg_integrator* h, const float* T, const float* depth, const uint8_t* label, int32_t width,
                                   int32_t height, const float* K) {
   if (!h || !T || !K || width <= 0 || height <= 0 || !depth || !label) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   const size_t P = (size_t)width * height;
-  if ((int64_t)P > h->cap_points) return fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");
+  if ((int64_t)P > h->cap_points) return h->fail(KSG_ERR_INVALID_ARGUMENT, "cloud / frame larger than ksg_config.max_points");
   const size_t o_lab = (P * 4 + 255) / 256 * 256;
   const size_t total = o_lab + (P + 255) / 256 * 256;
   const int slot = h->in_slot;
   h->in_slot ^= 1;
   if (total > h->in2_bytes[slot]) {
     if (h->in2_used[slot]) KSG_CUDA(cudaEventSynchronize(h->ev_free[slot]));
-    if (h->d_in2[slot]) cudaFree(h->d_in2[slot]);
-    if (h->h_stage2[slot]) cudaFreeHost(h->h_stage2[slot]);
-    h->d_in2[slot] = nullptr; h->h_stage2[slot] = nullptr;
-    KSG_CUDA(cudaMalloc((void**)&h->d_in2[slot], total));
-    KSG_CUDA(cudaMallocHost((void**)&h->h_stage2[slot], total));
-    h->in2_bytes[slot] = total;
+    h->res.release(h->h_stage2[slot]);   // both buffers of the slot go before either is replaced
+    h->h_stage2[slot] = nullptr;
+    KSG_CUDA(h->res.regrow(&h->d_in2[slot], &h->in2_bytes[slot], total));
+    KSG_CUDA(h->res.regrow_pinned(&h->h_stage2[slot], &h->in2_bytes[slot], total));
   }
   // the slot's previous frame must have consumed the device buffer before it is overwritten
   if (h->in2_used[slot]) KSG_CUDA(cudaStreamWaitEvent(h->copy_stream, h->ev_free[slot], 0));
@@ -1545,20 +1657,16 @@ int64_t update_log_count(const ksg_integrator* h) {
 
 int32_t ksg_set_update_log(ksg_integrator* h, int64_t capacity_voxels) {
   if (!h || capacity_voxels < 0 || capacity_voxels > (1ll << 30)) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
-  if (h->d_log_head) cudaFree(h->d_log_head);
-  if (h->d_log_prior) cudaFree(h->d_log_prior);
-  if (h->h_log_head) cudaFreeHost(h->h_log_head);
-  if (h->h_log_prior) cudaFreeHost(h->h_log_prior);
+  for (void* p : {(void*)h->d_log_head, (void*)h->d_log_prior, (void*)h->h_log_head, (void*)h->h_log_prior}) h->res.release(p);
   h->d_log_head = nullptr; h->d_log_prior = nullptr; h->h_log_head = nullptr; h->h_log_prior = nullptr; h->log_cap = 0;
   h->merged_log_count = 0;
   if (capacity_voxels == 0) return KSG_OK;
   if (h->cfg.integrator_type == KSG_INTEGRATOR_MERGED) {
     // the merged log pass compacts the segment heads of up to rec_cap records in the unsorted record buffer (ksg_log.cuh)
-    if (h->rec_cap > 0x7fffffffll) return fail(KSG_ERR_INVALID_ARGUMENT, "update log: max_updates must be below 2^31 for the merged integrator");
+    if (h->rec_cap > 0x7fffffffll) return h->fail(KSG_ERR_INVALID_ARGUMENT, "update log: max_updates must be below 2^31 for the merged integrator");
     size_t t = 0, t2 = 0;
     KSG_CUDA(cub::DeviceSelect::Flagged(nullptr, t, cub::CountingInputIterator<int>(0), (uint8_t*)nullptr, (int*)nullptr, (int*)nullptr,
                                         (int)h->rec_cap));
@@ -1566,31 +1674,25 @@ int32_t ksg_set_update_log(ksg_integrator* h, int64_t capacity_voxels) {
     cub::DoubleBuffer<int> vb(nullptr, nullptr);
     KSG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t2, kb, vb, (int)std::min<int64_t>(capacity_voxels, h->rec_cap), 0, 63));
     t = std::max(t, t2);
-    if (t > h->cub_temp_bytes) {
-      if (h->cub_temp) cudaFree(h->cub_temp);
-      h->cub_temp = nullptr; h->cub_temp_bytes = 0;
-      KSG_CUDA(cudaMalloc(&h->cub_temp, t + 256));
-      h->cub_temp_bytes = t + 256;
-    }
+    if (t > h->cub_temp_bytes) KSG_CUDA(h->res.regrow(&h->cub_temp, &h->cub_temp_bytes, t + 256));
   }
   const size_t n = (size_t)capacity_voxels;
-  KSG_CUDA(cudaMalloc((void**)&h->d_log_head, n * sizeof(VoxelUpdate)));
-  KSG_CUDA(cudaMalloc((void**)&h->d_log_prior, n * sizeof(float) * h->dc.C));
-  KSG_CUDA(cudaMallocHost((void**)&h->h_log_head, n * sizeof(VoxelUpdate)));
-  KSG_CUDA(cudaMallocHost((void**)&h->h_log_prior, n * sizeof(float) * h->dc.C));
+  KSG_CUDA(h->res.device(&h->d_log_head, n));
+  KSG_CUDA(h->res.device(&h->d_log_prior, n * h->dc.C));
+  KSG_CUDA(h->res.pinned(&h->h_log_head, n));
+  KSG_CUDA(h->res.pinned(&h->h_log_prior, n * h->dc.C));
   h->log_cap = (int)capacity_voxels;
   return KSG_OK;
 }
 
 int32_t ksg_fetch_update_log(ksg_integrator* h, int64_t* n_out, const ksg_voxel_update** heads, const float** priors) {
   if (!h || !n_out) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   *n_out = 0;
-  if (!h->d_log_head) return fail(KSG_ERR_INVALID_ARGUMENT, "update log is off (ksg_set_update_log)");
+  if (!h->d_log_head) return h->fail(KSG_ERR_INVALID_ARGUMENT, "update log is off (ksg_set_update_log)");
   KSG_CUDA(cudaSetDevice(h->device));
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
   const int64_t n = update_log_count(h);
-  if (n > h->log_cap) { *n_out = -1; return fail(KSG_ERR_SCRATCH_FULL, "update log too small for this frame: fall back to ksg_last_updated_blocks / ksg_export_blocks_by_index"); }
+  if (n > h->log_cap) { *n_out = -1; return h->fail(KSG_ERR_SCRATCH_FULL, "update log too small for this frame: fall back to ksg_last_updated_blocks / ksg_export_blocks_by_index"); }
   if (n > 0) {
     KSG_CUDA(cudaMemcpyAsync(h->h_log_head, h->d_log_head, (size_t)n * sizeof(VoxelUpdate), cudaMemcpyDeviceToHost, h->own_stream));
     KSG_CUDA(cudaMemcpyAsync(h->h_log_prior, h->d_log_prior, (size_t)n * sizeof(float) * h->dc.C, cudaMemcpyDeviceToHost, h->own_stream));
@@ -1606,16 +1708,16 @@ int32_t ksg_evaluate_labels(ksg_integrator* h, const ksg_world_object* objects, 
                             float checker_margin, int64_t* evaluated, int64_t* correct, int64_t* observed) {
   if (!h || n_objects < 0 || (n_objects > 0 && !objects) || n_objects > 4096) return KSG_ERR_INVALID_ARGUMENT;
   static_assert(sizeof(ksg_world_object) == sizeof(WorldObject), "ksg_world_object layout");
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
   unsigned long long res[3] = {0, 0, 0};
   if (h->num_blocks > 0 && n_objects > 0) {
+    Resources tmp;
     WorldObject* d_objs = nullptr;
     unsigned long long* d_out = nullptr;
-    KSG_CUDA(cudaMalloc((void**)&d_objs, sizeof(WorldObject) * (size_t)n_objects));
-    KSG_CUDA(cudaMalloc((void**)&d_out, sizeof(res)));
+    KSG_CUDA(tmp.device(&d_objs, (size_t)n_objects));
+    KSG_CUDA(tmp.device(&d_out, 3));
     KSG_CUDA(cudaMemcpy(d_objs, objects, sizeof(WorldObject) * (size_t)n_objects, cudaMemcpyHostToDevice));
     KSG_CUDA(cudaMemset(d_out, 0, sizeof(res)));
     ++h->n_launches;
@@ -1623,7 +1725,6 @@ int32_t ksg_evaluate_labels(ksg_integrator* h, const ksg_world_object* objects, 
                                                               checker_margin, d_out);
     KSG_CUDA(cudaMemcpyAsync(res, d_out, sizeof(res), cudaMemcpyDeviceToHost, h->own_stream));
     KSG_CUDA(cudaStreamSynchronize(h->own_stream));
-    cudaFree(d_objs); cudaFree(d_out);
   }
   if (evaluated) *evaluated = (int64_t)res[0];
   if (correct) *correct = (int64_t)res[1];
@@ -1631,12 +1732,104 @@ int32_t ksg_evaluate_labels(ksg_integrator* h, const ksg_world_object* objects, 
   return KSG_OK;
 }
 
-static bool key_less_zyx(uint64_t a, uint64_t b);
+namespace {
+// Host copy of the block hash table (ht_keys / ht_slot), probed exactly as the device probes it: linear probing from mix64(key).
+struct HostBlockTable {
+  std::vector<uint64_t> keys;
+  std::vector<int> slot_of;
+  uint32_t mask = 0;
+
+  int load(ksg_integrator* h) {
+    mask = h->map.ht_mask;
+    keys.resize((size_t)h->ht_cap);
+    slot_of.resize((size_t)h->ht_cap);
+    KSG_CUDA(cudaMemcpy(keys.data(), h->map.ht_keys, sizeof(uint64_t) * h->ht_cap, cudaMemcpyDeviceToHost));
+    KSG_CUDA(cudaMemcpy(slot_of.data(), h->map.ht_slot, sizeof(int) * h->ht_cap, cudaMemcpyDeviceToHost));
+    return KSG_OK;
+  }
+  int store(ksg_integrator* h) const {
+    KSG_CUDA(cudaMemcpy(h->map.ht_keys, keys.data(), sizeof(uint64_t) * h->ht_cap, cudaMemcpyHostToDevice));
+    KSG_CUDA(cudaMemcpy(h->map.ht_slot, slot_of.data(), sizeof(int) * h->ht_cap, cudaMemcpyHostToDevice));
+    return KSG_OK;
+  }
+  // The slot of `key`, or -1.
+  int find(uint64_t key) const {
+    const uint32_t pos = probe(key);
+    return (pos != kNone && keys[pos] == key) ? slot_of[pos] : -1;
+  }
+  // The slot of `key`; an absent key takes slot *n_blocks, which then grows by one.  -1: the table or the pool is full.
+  int find_or_insert(uint64_t key, int64_t* n_blocks, int64_t max_blocks) {
+    const uint32_t pos = probe(key);
+    if (pos == kNone) return -1;
+    if (keys[pos] == key) return slot_of[pos];
+    if (*n_blocks >= max_blocks) return -1;
+    keys[pos] = key; slot_of[pos] = (int)*n_blocks;
+    return (int)(*n_blocks)++;
+  }
+
+ private:
+  static constexpr uint32_t kNone = 0xFFFFFFFFu;
+  // where `key` is, or the empty entry that ends its probe sequence; kNone: every entry probed
+  uint32_t probe(uint64_t key) const {
+    uint32_t pos = mix64(key) & mask;
+    for (uint32_t n = 0; n <= mask; ++n) {
+      if (keys[pos] == key || keys[pos] == kEmptyKey) return pos;
+      pos = (pos + 1) & mask;
+    }
+    return kNone;
+  }
+};
+
+void put_block_index(int32_t* block_index, int64_t i, uint64_t key) {
+  const I3 b = unpack_key(key);
+  block_index[3 * i] = b.x; block_index[3 * i + 1] = b.y; block_index[3 * i + 2] = b.z;
+}
+
+// The pool slots of the map's blocks in (z, y, x) order (keys are packed as z:y:x, biased: numeric order = (z, y, x)), and,
+// where block_index is given, the blocks' indices in that order.
+int slots_zyx(ksg_integrator* h, std::vector<int>* order, int32_t* block_index) {
+  const int64_t nb = h->num_blocks;
+  std::vector<uint64_t> keys((size_t)nb);
+  KSG_CUDA(cudaMemcpy(keys.data(), h->map.slot_key, sizeof(uint64_t) * nb, cudaMemcpyDeviceToHost));
+  order->resize((size_t)nb);
+  for (int64_t i = 0; i < nb; ++i) (*order)[i] = (int)i;
+  std::sort(order->begin(), order->end(), [&](int a, int b) { return keys[a] < keys[b]; });
+  if (block_index) for (int64_t i = 0; i < nb; ++i) put_block_index(block_index, i, keys[(*order)[i]]);
+  return KSG_OK;
+}
+
+// Staging of ksg_export_blocks / ksg_import_blocks in d_exp, per batch of `cnt` blocks:
+// [distance | weight | rgba | semantic rgba | priors | labels | (import) fresh-block flags], batches of at most 256 MiB.
+struct BlockStaging {
+  size_t VB, C, per_block;
+  int64_t batch;
+  BlockStaging(const DevCfg& dc, int64_t n)
+      : VB((size_t)dc.vps * dc.vps * dc.vps), C((size_t)dc.C), per_block(VB * (4 + 4 + 4 + 1 + 4 + 4 * C) + 64),
+        batch(std::max<int64_t>(1, std::min<int64_t>(n, (int64_t)((256ull << 20) / per_block)))) {}
+  struct Parts { float* dist; float* wgt; uint32_t* rgba; uint32_t* srgba; float* prior; uint8_t* label; uint8_t* fresh; };
+  Parts at(uint8_t* p, int64_t cnt) const {
+    Parts q;
+    q.dist = (float*)p; p += cnt * VB * 4;
+    q.wgt = (float*)p; p += cnt * VB * 4;
+    q.rgba = (uint32_t*)p; p += cnt * VB * 4;
+    q.srgba = (uint32_t*)p; p += cnt * VB * 4;
+    q.prior = (float*)p; p += cnt * VB * 4 * C;
+    q.label = p; p += cnt * VB;
+    q.fresh = p;
+    return q;
+  }
+  // the slot list and the staging buffer for one batch; `bytes` is batch * per_block, plus the flags for an import
+  int ensure(ksg_integrator* h, size_t bytes) const {
+    if (h->exp_slots_cap < batch) KSG_CUDA(h->res.regrow(&h->d_exp_slots, &h->exp_slots_cap, (size_t)batch));
+    if (h->d_exp_bytes < bytes) KSG_CUDA(h->res.regrow(&h->d_exp, &h->d_exp_bytes, bytes));
+    return KSG_OK;
+  }
+};
+}  // namespace
 
 int32_t ksg_extract_mesh(ksg_integrator* h, float min_weight, int64_t vertex_capacity, float* vertices, uint8_t* rgba, uint8_t* labels,
                          int64_t block_capacity, int32_t* block_index, int64_t* block_first_vertex, int64_t* n_vertices, int64_t* n_blocks) {
   if (!h || vertex_capacity < 0 || block_capacity < 0) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
@@ -1644,58 +1837,47 @@ int32_t ksg_extract_mesh(ksg_integrator* h, float min_weight, int64_t vertex_cap
   if (n_blocks) *n_blocks = nb;
   if (n_vertices) *n_vertices = 0;
   if (nb == 0) { if (block_first_vertex && block_capacity >= 0) block_first_vertex[0] = 0; return KSG_OK; }
-  if ((block_index || block_first_vertex) && nb > block_capacity) return fail(KSG_ERR_INVALID_ARGUMENT, "mesh: block capacity too small");
+  if ((block_index || block_first_vertex) && nb > block_capacity) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh: block capacity too small");
   // blocks in (z, y, x) order, as ksg_export_blocks lists them
-  std::vector<uint64_t> keys((size_t)nb);
-  KSG_CUDA(cudaMemcpy(keys.data(), h->map.slot_key, sizeof(uint64_t) * nb, cudaMemcpyDeviceToHost));
-  std::vector<int> order((size_t)nb);
-  for (int64_t i = 0; i < nb; ++i) order[i] = (int)i;
-  std::sort(order.begin(), order.end(), [&](int a, int b) { return key_less_zyx(keys[a], keys[b]); });
+  std::vector<int> order;
+  { const int rco = slots_zyx(h, &order, block_index); if (rco) return rco; }
+  Resources tmp;
   int* d_slots = nullptr; int* d_count = nullptr; long long* d_first = nullptr;
-  float* d_vtx = nullptr; uint32_t* d_rgba = nullptr; uint8_t* d_label = nullptr;
-  auto release = [&]() { cudaFree(d_slots); cudaFree(d_count); cudaFree(d_first); cudaFree(d_vtx); cudaFree(d_rgba); cudaFree(d_label); };
-#define KSG_MESH(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { release(); return fail(KSG_ERR_CUDA, cudaGetErrorString(e_)); } } while (0)
-  KSG_MESH(cudaMalloc((void**)&d_slots, sizeof(int) * nb));
-  KSG_MESH(cudaMalloc((void**)&d_count, sizeof(int) * nb));
-  KSG_MESH(cudaMalloc((void**)&d_first, sizeof(long long) * nb));
-  KSG_MESH(cudaMemcpy(d_slots, order.data(), sizeof(int) * nb, cudaMemcpyHostToDevice));
+  KSG_CUDA(tmp.device(&d_slots, nb));
+  KSG_CUDA(tmp.device(&d_count, nb));
+  KSG_CUDA(tmp.device(&d_first, nb));
+  KSG_CUDA(cudaMemcpy(d_slots, order.data(), sizeof(int) * nb, cudaMemcpyHostToDevice));
   cudaStream_t s = h->own_stream;
   const int grid = (int)std::min<int64_t>(nb, (int64_t)h->sm_count * 8);
   MeshBuf none{nullptr, nullptr, nullptr};
   ++h->n_launches;
   k_mesh_blocks<false><<<grid, kMeshThreads, 0, s>>>(h->dc, h->map, d_slots, (int)nb, min_weight, nullptr, d_count, none);
   std::vector<int> count((size_t)nb);
-  KSG_MESH(cudaMemcpyAsync(count.data(), d_count, sizeof(int) * nb, cudaMemcpyDeviceToHost, s));
-  KSG_MESH(cudaStreamSynchronize(s));
+  KSG_CUDA(cudaMemcpyAsync(count.data(), d_count, sizeof(int) * nb, cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
   std::vector<long long> first((size_t)nb + 1);
   first[0] = 0;
   for (int64_t i = 0; i < nb; ++i) first[i + 1] = first[i] + count[i];
   const int64_t total = first[nb];
   if (n_vertices) *n_vertices = total;
-  if (block_index)
-    for (int64_t i = 0; i < nb; ++i) {
-      const I3 b = unpack_key(keys[order[i]]);
-      block_index[3 * i] = b.x; block_index[3 * i + 1] = b.y; block_index[3 * i + 2] = b.z;
-    }
   if (block_first_vertex) for (int64_t i = 0; i <= nb && i <= block_capacity; ++i) block_first_vertex[i] = first[i];
-  if (!vertices && !rgba && !labels) { release(); return KSG_OK; }                 // counting call
-  if (total > vertex_capacity) { release(); return fail(KSG_ERR_INVALID_ARGUMENT, "mesh: vertex capacity too small (n_vertices holds the need)"); }
+  if (!vertices && !rgba && !labels) return KSG_OK;                 // counting call
+  if (total > vertex_capacity) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh: vertex capacity too small (n_vertices holds the need)");
   if (total > 0) {
-    KSG_MESH(cudaMalloc((void**)&d_vtx, sizeof(float) * 3 * total));
-    KSG_MESH(cudaMalloc((void**)&d_rgba, sizeof(uint32_t) * total));
-    KSG_MESH(cudaMalloc((void**)&d_label, (size_t)total));
-    KSG_MESH(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * nb, cudaMemcpyHostToDevice, s));
+    float* d_vtx = nullptr; uint32_t* d_rgba = nullptr; uint8_t* d_label = nullptr;
+    KSG_CUDA(tmp.device(&d_vtx, 3 * (size_t)total));
+    KSG_CUDA(tmp.device(&d_rgba, (size_t)total));
+    KSG_CUDA(tmp.device(&d_label, (size_t)total));
+    KSG_CUDA(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * nb, cudaMemcpyHostToDevice, s));
     MeshBuf mb{d_vtx, d_rgba, d_label};
     ++h->n_launches;
     k_mesh_blocks<true><<<grid, kMeshThreads, 0, s>>>(h->dc, h->map, d_slots, (int)nb, min_weight, d_first, nullptr, mb);
-    if (vertices) KSG_MESH(cudaMemcpyAsync(vertices, d_vtx, sizeof(float) * 3 * total, cudaMemcpyDeviceToHost, s));
-    if (rgba) KSG_MESH(cudaMemcpyAsync(rgba, d_rgba, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost, s));
-    if (labels) KSG_MESH(cudaMemcpyAsync(labels, d_label, (size_t)total, cudaMemcpyDeviceToHost, s));
-    KSG_MESH(cudaStreamSynchronize(s));
-    KSG_MESH(cudaGetLastError());
+    if (vertices) KSG_CUDA(cudaMemcpyAsync(vertices, d_vtx, sizeof(float) * 3 * total, cudaMemcpyDeviceToHost, s));
+    if (rgba) KSG_CUDA(cudaMemcpyAsync(rgba, d_rgba, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost, s));
+    if (labels) KSG_CUDA(cudaMemcpyAsync(labels, d_label, (size_t)total, cudaMemcpyDeviceToHost, s));
+    KSG_CUDA(cudaStreamSynchronize(s));
+    KSG_CUDA(cudaGetLastError());
   }
-#undef KSG_MESH
-  release();
   return KSG_OK;
 }
 
@@ -1723,7 +1905,6 @@ void launch_query(ksg_integrator* h, int64_t n, const float* d_xyz, float min_we
 int32_t ksg_query_points(ksg_integrator* h, int64_t n, const float* xyz_G, float min_weight, const ksg_query_out* out) {
   bool work = false;
   { const int rca = query_args(h, n, xyz_G, min_weight, out, &work); if (rca) return rca; }
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
@@ -1736,23 +1917,20 @@ int32_t ksg_query_points(ksg_integrator* h, int64_t n, const float* xyz_G, float
                             o.gradient ? 12 * N : 0};
   size_t off[10], total = 0;
   for (int k = 0; k < 10; ++k) { off[k] = total; total += (sizes[k] + 255) / 256 * 256; }
+  Resources tmp;
   uint8_t* d = nullptr;
-  KSG_CUDA(cudaMalloc((void**)&d, total));
+  KSG_CUDA(tmp.device(&d, total));
   auto at = [&](int k) -> void* { return sizes[k] ? (void*)(d + off[k]) : nullptr; };
   ksg_query_out dq{(uint8_t*)at(1), (float*)at(2), (float*)at(3), (uint8_t*)at(4), (uint8_t*)at(5), (float*)at(6), (uint8_t*)at(7),
                    (float*)at(8), (float*)at(9)};
   void* host[10] = {nullptr, o.flags, o.tsdf_distance, o.tsdf_weight, o.tsdf_rgba, o.sem_label, o.sem_priors, o.sem_rgba, o.distance, o.gradient};
   cudaStream_t s = h->own_stream;
-  cudaError_t e = cudaMemcpyAsync(d, xyz_G, sizes[0], cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) {
-    launch_query(h, n, (const float*)d, min_weight, dq, s);
-    e = cudaGetLastError();
-  }
-  for (int k = 1; k < 10 && e == cudaSuccess; ++k)
-    if (sizes[k]) e = cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFree(d);
-  if (e != cudaSuccess) return fail(KSG_ERR_CUDA, cudaGetErrorString(e));
+  KSG_CUDA(cudaMemcpyAsync(d, xyz_G, sizes[0], cudaMemcpyHostToDevice, s));
+  launch_query(h, n, (const float*)d, min_weight, dq, s);
+  KSG_CUDA(cudaGetLastError());
+  for (int k = 1; k < 10; ++k)
+    if (sizes[k]) KSG_CUDA(cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
 }
 
@@ -1760,7 +1938,6 @@ int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz
                                 void* cuda_stream) {
   bool work = false;
   { const int rca = query_args(h, n, d_xyz_G, min_weight, d_out, &work); if (rca) return rca; }
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
   if (!work) return KSG_OK;
   KSG_CUDA(cudaSetDevice(h->device));
@@ -1771,7 +1948,6 @@ int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz
 
 int32_t ksg_sync(ksg_integrator* h) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
@@ -1785,51 +1961,29 @@ int64_t ksg_num_blocks(ksg_integrator* h) {
   return h->num_blocks;
 }
 
-static bool key_less_zyx(uint64_t a, uint64_t b) { return a < b; }  // packed as z:y:x, biased -> numeric order = (z, y, x)
-
 static int export_slots(ksg_integrator* h, const std::vector<int>& slots, float* tsdf_distance, float* tsdf_weight,
                         uint8_t* tsdf_rgba, uint8_t* sem_label, float* sem_priors, uint8_t* sem_rgba) {
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   const int64_t nb = (int64_t)slots.size();
   if (nb == 0) return KSG_OK;
   const DevCfg& dc = h->dc;
-  const size_t VB = (size_t)dc.vps * dc.vps * dc.vps;
-  const size_t per_block = VB * (4 + 4 + 4 + 1 + 4 + 4 * (size_t)dc.C) + 64;
-  const int64_t batch = std::max<int64_t>(1, std::min<int64_t>(nb, (int64_t)((256ull << 20) / per_block)));
-  if (h->exp_slots_cap < batch) {
-    if (h->d_exp_slots) cudaFree(h->d_exp_slots);
-    h->d_exp_slots = nullptr;
-    KSG_CUDA(dmalloc(&h->d_exp_slots, (size_t)batch));
-    h->exp_slots_cap = (int)batch;
-  }
-  const size_t need = (size_t)batch * per_block;
-  if (h->d_exp_bytes < need) {
-    if (h->d_exp) cudaFree(h->d_exp);
-    h->d_exp = nullptr;
-    KSG_CUDA(cudaMalloc((void**)&h->d_exp, need));
-    h->d_exp_bytes = need;
-  }
-  for (int64_t b0 = 0; b0 < nb; b0 += batch) {
-    const int64_t cnt = std::min(batch, nb - b0);
+  const BlockStaging st(dc, nb);
+  const size_t VB = st.VB;
+  { const int rcs = st.ensure(h, (size_t)st.batch * st.per_block); if (rcs) return rcs; }
+  for (int64_t b0 = 0; b0 < nb; b0 += st.batch) {
+    const int64_t cnt = std::min(st.batch, nb - b0);
     KSG_CUDA(cudaMemcpy(h->d_exp_slots, slots.data() + b0, sizeof(int) * cnt, cudaMemcpyHostToDevice));
-    uint8_t* p = h->d_exp;
-    float* o_dist = (float*)p; p += cnt * VB * 4;
-    float* o_wgt = (float*)p; p += cnt * VB * 4;
-    uint32_t* o_rgba = (uint32_t*)p; p += cnt * VB * 4;
-    uint32_t* o_srgba = (uint32_t*)p; p += cnt * VB * 4;
-    float* o_prior = (float*)p; p += cnt * VB * 4 * dc.C;
-    uint8_t* o_label = p;
-    k_export<<<h->sm_count * 4, 256, 0, h->own_stream>>>(dc, h->map, h->d_exp_slots, (int)cnt, tsdf_distance ? o_dist : nullptr,
-                                                         tsdf_weight ? o_wgt : nullptr, tsdf_rgba ? o_rgba : nullptr,
-                                                         sem_label ? o_label : nullptr, sem_priors ? o_prior : nullptr,
-                                                         sem_rgba ? o_srgba : nullptr);
+    const BlockStaging::Parts o = st.at(h->d_exp, cnt);
+    k_export<<<h->sm_count * 4, 256, 0, h->own_stream>>>(dc, h->map, h->d_exp_slots, (int)cnt, tsdf_distance ? o.dist : nullptr,
+                                                         tsdf_weight ? o.wgt : nullptr, tsdf_rgba ? o.rgba : nullptr,
+                                                         sem_label ? o.label : nullptr, sem_priors ? o.prior : nullptr,
+                                                         sem_rgba ? o.srgba : nullptr);
     KSG_CUDA(cudaStreamSynchronize(h->own_stream));
-    if (tsdf_distance) KSG_CUDA(cudaMemcpy(tsdf_distance + b0 * VB, o_dist, cnt * VB * 4, cudaMemcpyDeviceToHost));
-    if (tsdf_weight) KSG_CUDA(cudaMemcpy(tsdf_weight + b0 * VB, o_wgt, cnt * VB * 4, cudaMemcpyDeviceToHost));
-    if (tsdf_rgba) KSG_CUDA(cudaMemcpy(tsdf_rgba + b0 * VB * 4, o_rgba, cnt * VB * 4, cudaMemcpyDeviceToHost));
-    if (sem_rgba) KSG_CUDA(cudaMemcpy(sem_rgba + b0 * VB * 4, o_srgba, cnt * VB * 4, cudaMemcpyDeviceToHost));
-    if (sem_label) KSG_CUDA(cudaMemcpy(sem_label + b0 * VB, o_label, cnt * VB, cudaMemcpyDeviceToHost));
-    if (sem_priors) KSG_CUDA(cudaMemcpy(sem_priors + b0 * VB * dc.C, o_prior, cnt * VB * 4 * dc.C, cudaMemcpyDeviceToHost));
+    if (tsdf_distance) KSG_CUDA(cudaMemcpy(tsdf_distance + b0 * VB, o.dist, cnt * VB * 4, cudaMemcpyDeviceToHost));
+    if (tsdf_weight) KSG_CUDA(cudaMemcpy(tsdf_weight + b0 * VB, o.wgt, cnt * VB * 4, cudaMemcpyDeviceToHost));
+    if (tsdf_rgba) KSG_CUDA(cudaMemcpy(tsdf_rgba + b0 * VB * 4, o.rgba, cnt * VB * 4, cudaMemcpyDeviceToHost));
+    if (sem_rgba) KSG_CUDA(cudaMemcpy(sem_rgba + b0 * VB * 4, o.srgba, cnt * VB * 4, cudaMemcpyDeviceToHost));
+    if (sem_label) KSG_CUDA(cudaMemcpy(sem_label + b0 * VB, o.label, cnt * VB, cudaMemcpyDeviceToHost));
+    if (sem_priors) KSG_CUDA(cudaMemcpy(sem_priors + b0 * VB * dc.C, o.prior, cnt * VB * 4 * dc.C, cudaMemcpyDeviceToHost));
   }
   return KSG_OK;
 }
@@ -1837,23 +1991,14 @@ static int export_slots(ksg_integrator* h, const std::vector<int>& slots, float*
 int32_t ksg_export_blocks(ksg_integrator* h, int64_t capacity_blocks, int32_t* block_index, float* tsdf_distance,
                           float* tsdf_weight, uint8_t* tsdf_rgba, uint8_t* sem_label, float* sem_priors, uint8_t* sem_rgba) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   finish_frame(h, nullptr);
   const int64_t nb = h->num_blocks;
-  if (nb > capacity_blocks) return fail(KSG_ERR_INVALID_ARGUMENT, "export capacity too small");
+  if (nb > capacity_blocks) return h->fail(KSG_ERR_INVALID_ARGUMENT, "export capacity too small");
   if (nb == 0) return KSG_OK;
-  std::vector<uint64_t> keys((size_t)nb);
-  KSG_CUDA(cudaMemcpy(keys.data(), h->map.slot_key, sizeof(uint64_t) * nb, cudaMemcpyDeviceToHost));
-  std::vector<int> order((size_t)nb);
-  for (int64_t i = 0; i < nb; ++i) order[i] = (int)i;
-  std::sort(order.begin(), order.end(), [&](int a, int b) { return key_less_zyx(keys[a], keys[b]); });
-  if (block_index)
-    for (int64_t i = 0; i < nb; ++i) {
-      const I3 b = unpack_key(keys[order[i]]);
-      block_index[3 * i] = b.x; block_index[3 * i + 1] = b.y; block_index[3 * i + 2] = b.z;
-    }
+  std::vector<int> order;
+  { const int rco = slots_zyx(h, &order, block_index); if (rco) return rco; }
   if (!tsdf_distance && !tsdf_weight && !tsdf_rgba && !sem_label && !sem_priors && !sem_rgba) return KSG_OK;
   return export_slots(h, order, tsdf_distance, tsdf_weight, tsdf_rgba, sem_label, sem_priors, sem_rgba);
 }
@@ -1861,30 +2006,17 @@ int32_t ksg_export_blocks(ksg_integrator* h, int64_t capacity_blocks, int32_t* b
 int32_t ksg_export_blocks_by_index(ksg_integrator* h, int64_t n, const int32_t* block_index, uint8_t* found, float* tsdf_distance,
                                    float* tsdf_weight, uint8_t* tsdf_rgba, uint8_t* sem_label, float* sem_priors, uint8_t* sem_rgba) {
   if (!h || n < 0 || (n > 0 && !block_index)) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   if (n == 0) return KSG_OK;
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   finish_frame(h, nullptr);
-  // host copy of the hash table: look the keys up exactly as the device does
-  std::vector<uint64_t> keys((size_t)h->ht_cap);
-  std::vector<int> slot_of((size_t)h->ht_cap);
-  KSG_CUDA(cudaMemcpy(keys.data(), h->map.ht_keys, sizeof(uint64_t) * h->ht_cap, cudaMemcpyDeviceToHost));
-  KSG_CUDA(cudaMemcpy(slot_of.data(), h->map.ht_slot, sizeof(int) * h->ht_cap, cudaMemcpyDeviceToHost));
+  HostBlockTable table;
+  { const int rct = table.load(h); if (rct) return rct; }
   std::vector<int> slots;
   std::vector<int64_t> where;
   for (int64_t i = 0; i < n; ++i) {
     I3 b; b.x = block_index[3 * i]; b.y = block_index[3 * i + 1]; b.z = block_index[3 * i + 2];
-    int slot = -1;
-    if (key_in_range(b)) {
-      const uint64_t key = pack_key(b);
-      uint32_t pos = mix64(key) & h->map.ht_mask;
-      for (uint32_t probe = 0; probe <= h->map.ht_mask; ++probe) {
-        if (keys[pos] == key) { slot = slot_of[pos]; break; }
-        if (keys[pos] == kEmptyKey) break;
-        pos = (pos + 1) & h->map.ht_mask;
-      }
-    }
+    const int slot = key_in_range(b) ? table.find(pack_key(b)) : -1;
     if (found) found[i] = slot >= 0 ? 1 : 0;
     if (slot >= 0) { slots.push_back(slot); where.push_back(i); }
   }
@@ -1915,84 +2047,52 @@ int32_t ksg_export_blocks_by_index(ksg_integrator* h, int64_t n, const int32_t* 
 int32_t ksg_import_blocks(ksg_integrator* h, int64_t n, const int32_t* block_index, const float* tsdf_distance, const float* tsdf_weight,
                           const uint8_t* tsdf_rgba, const uint8_t* sem_label, const float* sem_priors, const uint8_t* sem_rgba) {
   if (!h || n < 0 || (n > 0 && !block_index)) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
   if (n == 0) return KSG_OK;
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
   const DevCfg& dc = h->dc;
-  // host mirror of the block hash: look up / insert exactly as the device does (linear probing from mix64(key))
-  std::vector<uint64_t> keys((size_t)h->ht_cap);
-  std::vector<int> slot_of((size_t)h->ht_cap);
-  KSG_CUDA(cudaMemcpy(keys.data(), h->map.ht_keys, sizeof(uint64_t) * h->ht_cap, cudaMemcpyDeviceToHost));
-  KSG_CUDA(cudaMemcpy(slot_of.data(), h->map.ht_slot, sizeof(int) * h->ht_cap, cudaMemcpyDeviceToHost));
+  HostBlockTable table;
+  { const int rct = table.load(h); if (rct) return rct; }
   std::vector<int> slots((size_t)n);
   std::vector<uint8_t> fresh((size_t)n, 0);
   std::vector<uint64_t> new_keys;
   int64_t nb = h->num_blocks;
   for (int64_t i = 0; i < n; ++i) {
     I3 b; b.x = block_index[3 * i]; b.y = block_index[3 * i + 1]; b.z = block_index[3 * i + 2];
-    if (!key_in_range(b)) return fail(KSG_ERR_INDEX_RANGE, err_text(5));
+    if (!key_in_range(b)) return h->fail(KSG_ERR_INDEX_RANGE, err_text(5));
     const uint64_t key = pack_key(b);
-    uint32_t pos = mix64(key) & h->map.ht_mask;
-    for (uint32_t probe = 0;; ++probe) {
-      if (probe > h->map.ht_mask) return fail(KSG_ERR_POOL_FULL, err_text(3));
-      if (keys[pos] == key) { slots[i] = slot_of[pos]; break; }
-      if (keys[pos] == kEmptyKey) {
-        if (nb >= h->map.max_blocks) return fail(KSG_ERR_POOL_FULL, err_text(3));
-        keys[pos] = key; slot_of[pos] = (int)nb; slots[i] = (int)nb; fresh[i] = 1; new_keys.push_back(key); ++nb;
-        break;
-      }
-      pos = (pos + 1) & h->map.ht_mask;
-    }
+    const int64_t before = nb;
+    slots[i] = table.find_or_insert(key, &nb, h->map.max_blocks);
+    if (slots[i] < 0) return h->fail(KSG_ERR_POOL_FULL, err_text(3));
+    if (nb != before) { fresh[i] = 1; new_keys.push_back(key); }
   }
   if (!new_keys.empty()) {
-    KSG_CUDA(cudaMemcpy(h->map.ht_keys, keys.data(), sizeof(uint64_t) * h->ht_cap, cudaMemcpyHostToDevice));
-    KSG_CUDA(cudaMemcpy(h->map.ht_slot, slot_of.data(), sizeof(int) * h->ht_cap, cudaMemcpyHostToDevice));
+    { const int rct = table.store(h); if (rct) return rct; }
     KSG_CUDA(cudaMemcpy(h->map.slot_key + h->num_blocks, new_keys.data(), sizeof(uint64_t) * new_keys.size(), cudaMemcpyHostToDevice));
     const int pc = (int)nb;
     KSG_CUDA(cudaMemcpy(&h->d_cnt->pool_count, &pc, sizeof(int), cudaMemcpyHostToDevice));
     h->num_blocks = nb;
   }
-  const size_t VB = (size_t)dc.vps * dc.vps * dc.vps;
-  const size_t per_block = VB * (4 + 4 + 4 + 1 + 4 + 4 * (size_t)dc.C) + 64;
-  const int64_t batch = std::max<int64_t>(1, std::min<int64_t>(n, (int64_t)((256ull << 20) / per_block)));
-  if (h->exp_slots_cap < batch) {
-    if (h->d_exp_slots) cudaFree(h->d_exp_slots);
-    h->d_exp_slots = nullptr;
-    KSG_CUDA(dmalloc(&h->d_exp_slots, (size_t)batch));
-    h->exp_slots_cap = (int)batch;
-  }
-  const size_t need = (size_t)batch * per_block + (size_t)batch;
-  if (h->d_exp_bytes < need) {
-    if (h->d_exp) cudaFree(h->d_exp);
-    h->d_exp = nullptr;
-    KSG_CUDA(cudaMalloc((void**)&h->d_exp, need));
-    h->d_exp_bytes = need;
-  }
-  for (int64_t b0 = 0; b0 < n; b0 += batch) {
-    const int64_t cnt = std::min(batch, n - b0);
+  const BlockStaging st(dc, n);
+  const size_t VB = st.VB;
+  { const int rcs = st.ensure(h, (size_t)st.batch * st.per_block + (size_t)st.batch); if (rcs) return rcs; }
+  for (int64_t b0 = 0; b0 < n; b0 += st.batch) {
+    const int64_t cnt = std::min(st.batch, n - b0);
     KSG_CUDA(cudaMemcpy(h->d_exp_slots, slots.data() + b0, sizeof(int) * cnt, cudaMemcpyHostToDevice));
-    uint8_t* p = h->d_exp;
-    float* i_dist = (float*)p; p += cnt * VB * 4;
-    float* i_wgt = (float*)p; p += cnt * VB * 4;
-    uint32_t* i_rgba = (uint32_t*)p; p += cnt * VB * 4;
-    uint32_t* i_srgba = (uint32_t*)p; p += cnt * VB * 4;
-    float* i_prior = (float*)p; p += cnt * VB * 4 * dc.C;
-    uint8_t* i_label = p; p += cnt * VB;
-    uint8_t* d_fresh = p;
-    if (tsdf_distance) KSG_CUDA(cudaMemcpy(i_dist, tsdf_distance + b0 * VB, cnt * VB * 4, cudaMemcpyHostToDevice));
-    if (tsdf_weight) KSG_CUDA(cudaMemcpy(i_wgt, tsdf_weight + b0 * VB, cnt * VB * 4, cudaMemcpyHostToDevice));
-    if (tsdf_rgba) KSG_CUDA(cudaMemcpy(i_rgba, tsdf_rgba + b0 * VB * 4, cnt * VB * 4, cudaMemcpyHostToDevice));
-    if (sem_rgba) KSG_CUDA(cudaMemcpy(i_srgba, sem_rgba + b0 * VB * 4, cnt * VB * 4, cudaMemcpyHostToDevice));
-    if (sem_label) KSG_CUDA(cudaMemcpy(i_label, sem_label + b0 * VB, cnt * VB, cudaMemcpyHostToDevice));
-    if (sem_priors) KSG_CUDA(cudaMemcpy(i_prior, sem_priors + b0 * VB * dc.C, cnt * VB * 4 * dc.C, cudaMemcpyHostToDevice));
-    KSG_CUDA(cudaMemcpy(d_fresh, fresh.data() + b0, cnt, cudaMemcpyHostToDevice));
-    k_import<<<h->sm_count * 4, 256, 0, h->own_stream>>>(dc, h->map, h->d_exp_slots, d_fresh, (int)cnt, tsdf_distance ? i_dist : nullptr,
-                                                         tsdf_weight ? i_wgt : nullptr, tsdf_rgba ? i_rgba : nullptr,
-                                                         sem_label ? i_label : nullptr, sem_priors ? i_prior : nullptr,
-                                                         sem_rgba ? i_srgba : nullptr);
+    const BlockStaging::Parts i = st.at(h->d_exp, cnt);
+    if (tsdf_distance) KSG_CUDA(cudaMemcpy(i.dist, tsdf_distance + b0 * VB, cnt * VB * 4, cudaMemcpyHostToDevice));
+    if (tsdf_weight) KSG_CUDA(cudaMemcpy(i.wgt, tsdf_weight + b0 * VB, cnt * VB * 4, cudaMemcpyHostToDevice));
+    if (tsdf_rgba) KSG_CUDA(cudaMemcpy(i.rgba, tsdf_rgba + b0 * VB * 4, cnt * VB * 4, cudaMemcpyHostToDevice));
+    if (sem_rgba) KSG_CUDA(cudaMemcpy(i.srgba, sem_rgba + b0 * VB * 4, cnt * VB * 4, cudaMemcpyHostToDevice));
+    if (sem_label) KSG_CUDA(cudaMemcpy(i.label, sem_label + b0 * VB, cnt * VB, cudaMemcpyHostToDevice));
+    if (sem_priors) KSG_CUDA(cudaMemcpy(i.prior, sem_priors + b0 * VB * dc.C, cnt * VB * 4 * dc.C, cudaMemcpyHostToDevice));
+    KSG_CUDA(cudaMemcpy(i.fresh, fresh.data() + b0, cnt, cudaMemcpyHostToDevice));
+    k_import<<<h->sm_count * 4, 256, 0, h->own_stream>>>(dc, h->map, h->d_exp_slots, i.fresh, (int)cnt, tsdf_distance ? i.dist : nullptr,
+                                                         tsdf_weight ? i.wgt : nullptr, tsdf_rgba ? i.rgba : nullptr,
+                                                         sem_label ? i.label : nullptr, sem_priors ? i.prior : nullptr,
+                                                         sem_rgba ? i.srgba : nullptr);
     KSG_CUDA(cudaStreamSynchronize(h->own_stream));
   }
   return KSG_OK;
@@ -2000,7 +2100,6 @@ int32_t ksg_import_blocks(ksg_integrator* h, int64_t n, const int32_t* block_ind
 
 int32_t ksg_device_map_view(ksg_integrator* h, int64_t* n_blocks, int64_t* block_stride_bytes, void** d_pool, void** d_block_keys) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
@@ -2013,7 +2112,6 @@ int32_t ksg_device_map_view(ksg_integrator* h, int64_t* n_blocks, int64_t* block
 
 int32_t ksg_copy_map_device(ksg_integrator* h, void* d_dst_pool, void* d_dst_keys, void* stream) {
   if (!h || !d_dst_pool || !d_dst_keys) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
   cudaStream_t s = stream ? (cudaStream_t)stream : h->own_stream;
@@ -2026,7 +2124,6 @@ int32_t ksg_copy_map_device(ksg_integrator* h, void* d_dst_pool, void* d_dst_key
 
 int32_t ksg_merge_blocks_device(ksg_integrator* h, int64_t n_blocks, const void* d_block_keys, const void* d_pool_src, void* stream) {
   if (!h || n_blocks < 0 || (n_blocks > 0 && (!d_block_keys || !d_pool_src))) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
   if (n_blocks == 0) return KSG_OK;
   KSG_CUDA(cudaSetDevice(h->device));
@@ -2034,10 +2131,7 @@ int32_t ksg_merge_blocks_device(ksg_integrator* h, int64_t n_blocks, const void*
   cudaStream_t s = stream ? (cudaStream_t)stream : h->own_stream;
   if (h->exp_slots_cap < n_blocks) {
     KSG_CUDA(cudaStreamSynchronize(s));
-    if (h->d_exp_slots) cudaFree(h->d_exp_slots);
-    h->d_exp_slots = nullptr;
-    KSG_CUDA(dmalloc(&h->d_exp_slots, (size_t)n_blocks));
-    h->exp_slots_cap = (int)n_blocks;
+    KSG_CUDA(h->res.regrow(&h->d_exp_slots, &h->exp_slots_cap, (size_t)n_blocks));
   }
   h->frame_stamp += 1;
   h->n_launches += 5;
@@ -2046,28 +2140,20 @@ int32_t ksg_merge_blocks_device(ksg_integrator* h, int64_t n_blocks, const void*
   k_block_init<<<h->sm_count * 4, 256, 0, s>>>(h->dc, h->d_cnt, h->map);
   k_frame_finish<<<1, 1, 0, s>>>(h->d_cnt, h->map);
   k_merge_tiles<<<h->sm_count * 8, 256, 0, s>>>(h->dc, h->d_cnt, h->map, h->d_luts, h->d_exp_slots, (const uint8_t*)d_pool_src, (int)n_blocks);
-  KSG_CUDA(cudaGetLastError());
-  int rc = fetch_counters(h, s);
-  if (rc) return rc;
-  h->num_blocks = h->h_cnt->pool_count;
-  h->last_blocks_touched = h->h_cnt->n_blocks_touched;
-  const int dev_err = h->h_cnt->err;
-  if (dev_err) { h->deferred_status = dev_err; return fail(dev_err, err_text(dev_err)); }
-  return KSG_OK;
+  return finish_sync(h, s);
 }
 
 int32_t ksg_copy_update_log_device(ksg_integrator* h, int64_t* n_out, void* d_dst_updates, void* d_dst_priors, int64_t capacity, void* stream) {
   if (!h || !n_out) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   *n_out = 0;
-  if (!h->d_log_head) return fail(KSG_ERR_INVALID_ARGUMENT, "update log is off (ksg_set_update_log)");
+  if (!h->d_log_head) return h->fail(KSG_ERR_INVALID_ARGUMENT, "update log is off (ksg_set_update_log)");
   KSG_CUDA(cudaSetDevice(h->device));
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
   const int64_t n = update_log_count(h);
-  if (n > h->log_cap) { *n_out = -1; return fail(KSG_ERR_SCRATCH_FULL, "update log too small for this frame"); }
+  if (n > h->log_cap) { *n_out = -1; return h->fail(KSG_ERR_SCRATCH_FULL, "update log too small for this frame"); }
   *n_out = n;
   if (!d_dst_updates && !d_dst_priors) return KSG_OK;                 // size query
-  if (n > capacity) return fail(KSG_ERR_INVALID_ARGUMENT, "update log copy: capacity too small");
+  if (n > capacity) return h->fail(KSG_ERR_INVALID_ARGUMENT, "update log copy: capacity too small");
   cudaStream_t s = stream ? (cudaStream_t)stream : h->own_stream;
   if (n > 0) {
     if (d_dst_updates) KSG_CUDA(cudaMemcpyAsync(d_dst_updates, h->d_log_head, (size_t)n * sizeof(VoxelUpdate), cudaMemcpyDeviceToDevice, s));
@@ -2079,7 +2165,6 @@ int32_t ksg_copy_update_log_device(ksg_integrator* h, int64_t* n_out, void* d_ds
 int32_t ksg_merge_voxels_device(ksg_integrator* h, int32_t n_deltas, const int64_t* counts, int64_t stride, const void* d_updates, const void* d_priors,
                                 void* stream) {
   if (!h || n_deltas < 0 || n_deltas > 16 || stride < 0 || (n_deltas > 0 && (!counts || !d_updates || !d_priors))) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
   MergeCounts mc{};
   int64_t any = 0;
@@ -2093,13 +2178,10 @@ int32_t ksg_merge_voxels_device(ksg_integrator* h, int32_t n_deltas, const int64
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
   cudaStream_t s = stream ? (cudaStream_t)stream : h->own_stream;
   const int64_t total = (int64_t)n_deltas * stride;
-  if (total > 0x7fffffff) return fail(KSG_ERR_INVALID_ARGUMENT, "merge: n_deltas * stride_entries exceeds 2^31 - 1");
+  if (total > 0x7fffffff) return h->fail(KSG_ERR_INVALID_ARGUMENT, "merge: n_deltas * stride_entries exceeds 2^31 - 1");
   if (h->exp_slots_cap < total) {
     KSG_CUDA(cudaStreamSynchronize(s));
-    if (h->d_exp_slots) cudaFree(h->d_exp_slots);
-    h->d_exp_slots = nullptr;
-    KSG_CUDA(dmalloc(&h->d_exp_slots, (size_t)total));
-    h->exp_slots_cap = (int)total;
+    KSG_CUDA(h->res.regrow(&h->d_exp_slots, &h->exp_slots_cap, (size_t)total));
   }
   h->frame_stamp += 1;
   h->n_launches += 4 + n_deltas;
@@ -2115,14 +2197,7 @@ int32_t ksg_merge_voxels_device(ksg_integrator* h, int32_t n_deltas, const int64
     k_mergev_apply<<<std::max(1, grid), 256, 0, s>>>(h->dc, h->map, h->d_luts, upd + (size_t)g * stride, pri + (size_t)g * stride * h->dc.C,
                                                     h->d_exp_slots + (size_t)g * stride, mc.n[g]);
   }
-  KSG_CUDA(cudaGetLastError());
-  int rc = fetch_counters(h, s);
-  if (rc) return rc;
-  h->num_blocks = h->h_cnt->pool_count;
-  h->last_blocks_touched = h->h_cnt->n_blocks_touched;
-  const int dev_err = h->h_cnt->err;
-  if (dev_err) { h->deferred_status = dev_err; return fail(dev_err, err_text(dev_err)); }
-  return KSG_OK;
+  return finish_sync(h, s);
 }
 
 int64_t ksg_last_updated_blocks(ksg_integrator* h, int64_t capacity_blocks, int32_t* block_index) {
@@ -2138,11 +2213,8 @@ int64_t ksg_last_updated_blocks(ksg_integrator* h, int64_t capacity_blocks, int3
   if (cudaMemcpy(all.data(), h->map.ht_keys, sizeof(uint64_t) * h->ht_cap, cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
   std::vector<uint64_t> keys((size_t)n);
   for (int64_t i = 0; i < n; ++i) keys[i] = all[pos[i]];
-  std::sort(keys.begin(), keys.end());
-  for (int64_t i = 0; i < n; ++i) {
-    const I3 b = unpack_key(keys[i]);
-    block_index[3 * i] = b.x; block_index[3 * i + 1] = b.y; block_index[3 * i + 2] = b.z;
-  }
+  std::sort(keys.begin(), keys.end());   // (z, y, x) order
+  for (int64_t i = 0; i < n; ++i) put_block_index(block_index, i, keys[i]);
   return n;
 }
 
@@ -2180,7 +2252,7 @@ int32_t ksg_owner_mask(int32_t voxels_per_side, int32_t shard_rank, int32_t shar
 int32_t ksg_set_profiling(ksg_integrator* h, int32_t enable) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
   cudaSetDevice(h->device);
-  if (enable && !h->ev[0]) for (auto& e : h->ev) cudaEventCreate(&e);
+  if (enable && !h->ev[0]) for (auto& e : h->ev) h->res.event(&e, cudaEventDefault);
   h->profiling = enable != 0;
   for (double& m : h->phase_ms) m = 0.0;
   h->prof_frames = 0; h->n_launches = 0; h->n_libcalls = 0;
@@ -2206,16 +2278,14 @@ int32_t ksg_debug_chain_sum(const float* terms, int64_t n, float s0, float* resu
   if (n < 0 || (n > 0 && !terms) || !result || !(s0 < 0.0f)) return KSG_ERR_INVALID_ARGUMENT;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { cudaGetLastError(); return KSG_ERR_NO_DEVICE; }
+  Resources tmp;
   float *d_terms = nullptr, *d_out = nullptr;
   int32_t rc = KSG_ERR_CUDA;
-  if (cudaMalloc((void**)&d_terms, sizeof(float) * (size_t)std::max<int64_t>(n, 1)) == cudaSuccess &&
-      cudaMalloc((void**)&d_out, sizeof(float)) == cudaSuccess &&
+  if (tmp.device(&d_terms, (size_t)n) == cudaSuccess && tmp.device(&d_out, 1) == cudaSuccess &&
       (n == 0 || cudaMemcpy(d_terms, terms, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess)) {
     k_chain_debug<<<1, 32>>>(d_terms, (long long)n, s0, d_out);
     if (cudaMemcpy(result, d_out, sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess) rc = KSG_OK;
   }
-  if (d_terms) cudaFree(d_terms);
-  if (d_out) cudaFree(d_out);
   return rc;
 }
 
@@ -2250,9 +2320,10 @@ int32_t ksg_debug_tsdf_batch(const ksg_config* cfg, int32_t wide, int64_t n, con
   tp.use_weight_dropoff = cfg->use_weight_dropoff; tp.use_sparsity = cfg->use_sparsity_compensation_factor;
   // one buffer: [sdf n][uw n][colour n][dist, weight, rgba]
   const size_t m = (size_t)std::max<int64_t>(n, 1);
+  Resources tmp;
   uint32_t* d = nullptr;
   int32_t rc = KSG_ERR_CUDA;
-  if (cudaMalloc((void**)&d, sizeof(uint32_t) * (3 * m + 3)) == cudaSuccess) {
+  if (tmp.device(&d, 3 * m + 3) == cudaSuccess) {
     float* d_sdf = (float*)d; float* d_uw = (float*)(d + m); uint32_t* d_col = d + 2 * m; uint32_t* d_state = d + 3 * m;
     uint32_t state[3];
     std::memcpy(&state[0], dist, 4); std::memcpy(&state[1], wgt, 4); state[2] = *rgba;
@@ -2270,14 +2341,12 @@ int32_t ksg_debug_tsdf_batch(const ksg_config* cfg, int32_t wide, int64_t n, con
         rc = KSG_OK;
       }
     }
-    cudaFree(d);
   }
   return rc;
 }
 
 int32_t ksg_debug_apply_routes(ksg_integrator* h, int64_t* out4) {
   if (!h || !out4) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   for (int i = 0; i < 4; ++i) out4[i] = 0;
@@ -2299,12 +2368,12 @@ int64_t ksg_debug_tile_times(ksg_integrator* h, int32_t enable, int64_t capacity
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
   if (enable && !h->tile_debug) {
-    if (cudaMalloc((void**)&h->tile_debug, sizeof(long long) * 2 * (size_t)h->tile_cap) != cudaSuccess) { h->tile_debug = nullptr; return 0; }
+    if (h->res.device(&h->tile_debug, 2 * (size_t)h->tile_cap) != cudaSuccess) { h->tile_debug = nullptr; return 0; }
   }
   const int64_t n = std::min<int64_t>(h->h_cnt->n_tiles, h->tile_cap);
   if (h->tile_debug && records_and_cycles && capacity >= n && n > 0)
     cudaMemcpy(records_and_cycles, h->tile_debug, sizeof(long long) * 2 * n, cudaMemcpyDeviceToHost);
-  if (!enable && h->tile_debug) { cudaFree(h->tile_debug); h->tile_debug = nullptr; }
+  if (!enable && h->tile_debug) { h->res.release(h->tile_debug); h->tile_debug = nullptr; }
   return n;
 }
 
@@ -2321,7 +2390,6 @@ int64_t ksg_debug_fast_timeline(ksg_integrator* h, int64_t* out64, int64_t* swee
 
 int32_t ksg_clear_map(ksg_integrator* h) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
-  auto fail = [&](int c, const char* m) { return h->fail(c, m); };
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
