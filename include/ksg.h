@@ -89,7 +89,8 @@ typedef struct ksg_config {
   int32_t max_points;                  /* largest cloud / frame (pixels) accepted */
   int64_t max_ray_steps;               /* scratch: upper bound on ray-step candidates per frame */
   int64_t max_updates;                 /* scratch: upper bound on voxel updates per frame */
-  int32_t apply_mode;                  /* 0 = TMA-staged tile apply (default), 1 = cooperative-copy staging */
+  int32_t apply_mode;                  /* merged: 0 = per-voxel apply kernels (default), 1 = tile kernel with cooperative-copy
+                                        * staging.  fast ignores it: its voxel update stages no tiles (one warp per voxel) */
   /* spatial hash-block sharding of ONE map over several GPUs (SURVEY.md 8e): every rank receives every frame and casts every
    * ray, but applies only the 8^3 tiles it owns (owner = f(block index, tile)); results per voxel are identical to the
    * unsharded run. shard_count <= 1: off. */

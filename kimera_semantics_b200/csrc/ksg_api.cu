@@ -301,7 +301,10 @@ struct ksg_integrator {
   uint32_t* keys32 = nullptr;
   int *tile_cnt = nullptr, *tile_slot = nullptr;
   TileDesc* tile_list = nullptr;
-  int solve_grid = 0, apply_fast_smem = 0;
+  FastTile* fast_tiles = nullptr;    // [tile_cap]
+  FastItem* fast_items = nullptr;    // [item_cap] touched voxels of the frame
+  int item_cap = 0;
+  int solve_grid = 0, group_grid = 0, fast_apply_grid = 0;
   int solve_threads = 0;             // Knobs
   RayRec* rayrec = nullptr;
   int* wl = nullptr;                 // [3][max_points] per-ray listed sweep, two scan lists
@@ -620,7 +623,7 @@ int advance_sets(ksg_integrator* h, cudaStream_t s) {
   return KSG_OK;
 }
 
-// `fast` frame driver: five launches, no host read-back inside the frame (ksg_fast.cuh).
+// `fast` frame driver: six launches, no host read-back inside the frame (ksg_fast.cuh).
 int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, const Xform& T, int cap, cudaStream_t s,
                    ksg_frame_stats* stats) {
   const bool sorted = h->cfg.integration_order_mode == KSG_ORDER_SORTED;
@@ -692,13 +695,10 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   {
     ApplySrc src{};
     src.param = h->ray_param; src.label = h->ray_label; src.color = h->ray_color; src.tmp = nullptr;
-    const int ctas_per_sm = std::max(1, std::min(8, (int)(220 * 1024 / std::max(1, h->apply_fast_smem + 1024))));
-    const int grid = h->sm_count * ctas_per_sm;
-    ++h->n_launches;
-    with_tma(h->use_tma, [&](auto tma) {
-      with_nch(h->apply_nch, [&](auto nch) {
-        k_tile_apply_fast<decltype(tma)::value, decltype(nch)::value><<<grid, 512, h->apply_fast_smem, s>>>(f, src);
-      });
+    h->n_launches += 2;
+    k_fast_group<<<h->group_grid, kGroupThreads, 0, s>>>(f, h->fast_items, h->fast_tiles, h->item_cap);
+    with_nch(h->apply_nch, [&](auto nch) {
+      k_fast_apply<decltype(nch)::value><<<h->fast_apply_grid, kFastApplyThreads, 0, s>>>(f, src, h->fast_items, h->fast_tiles, h->item_cap);
     });
   }
   if (h->profiling) cudaEventRecord(h->ev[3], s);
@@ -1354,8 +1354,10 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     }
   }
   h->rec_cap = rec_cap;
-  KSG_CUDA(res.device(&h->rec_a, (size_t)rec_cap)); KSG_CUDA(res.device(&h->rec_b, (size_t)rec_cap));
-  h->vq.short_items = (unsigned long long*)h->rec_a;   // the unsorted record buffer is free once the sort has run
+  if (!fast) {     // merged's 64-bit records (fast keeps 32-bit keys in per-tile segments and its work items instead)
+    KSG_CUDA(res.device(&h->rec_a, (size_t)rec_cap)); KSG_CUDA(res.device(&h->rec_b, (size_t)rec_cap));
+    h->vq.short_items = (unsigned long long*)h->rec_a;   // the unsorted record buffer is free once the sort has run
+  }
   h->tile_cap = (long long)std::min<unsigned long long>((unsigned long long)cfg->max_blocks * dc.tiles_per_block, (unsigned long long)rec_cap);
   KSG_CUDA(res.device(&h->tile_begin, (size_t)h->tile_cap));
 
@@ -1417,14 +1419,20 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
       if (cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, h->device) == cudaSuccess && khz > 0) h->clock_khz = khz;
     }
     {
-      const size_t stage = dc.head_bytes + (dc.full_stage ? dc.prior_bytes : 0u);
-      h->apply_fast_smem = (int)(stage + (size_t)dc.tile_voxels * 10 + 16 + 2 * sizeof(uint32_t) * kFastKeyCap + 64 + 32 + (size_t)kFastPref * 21);
-      rc = for_each_tma_nch([&](auto tma, auto nch) -> int {
-        KSG_CUDA(cudaFuncSetAttribute(k_tile_apply_fast<decltype(tma)::value, decltype(nch)::value>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, h->apply_fast_smem));
+      // voxel update: k_fast_group sorts each touched tile's keys and lists its voxels as work items, k_fast_apply takes them a warp
+      // each.  A frame's items number at most its records and at most 512 per tile.
+      KSG_CUDA(res.device(&h->fast_tiles, (size_t)h->tile_cap));
+      h->item_cap = (int)std::min<long long>({rec_cap, h->tile_cap * dc.tile_voxels, (long long)INT_MAX});
+      KSG_CUDA(res.device(&h->fast_items, (size_t)h->item_cap));
+      int per_sm = 0;
+      KSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fast_group, kGroupThreads, 0));
+      h->group_grid = h->sm_count * std::max(1, per_sm);
+      rc = with_nch(h->apply_nch, [&](auto nch) -> int {
+        KSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fast_apply<decltype(nch)::value>, kFastApplyThreads, 0));
         return KSG_OK;
       });
       if (rc) return rc;
+      h->fast_apply_grid = h->sm_count * std::max(1, per_sm);
     }
   }
   KSG_CUDA(cudaDeviceSynchronize());
