@@ -139,32 +139,24 @@ class Resources {
   std::vector<Item> held_;
 };
 
-// Development knobs (environment), read once when an integrator is created.  They select experiments and shapes that were
-// measured against the defaults; ksg_create applies each one only where it mattered before (see there).
+// Development knobs (environment), read once when an integrator is created.  They reshape launches that were measured against
+// the defaults; ksg_create applies each one only where it mattered before (see there).
 //
-// KSG_HOT_KERNEL=1 and KSG_EMIT_WARP=1 were both slower than what they were meant to replace when they were written (the hot
-// voxels' critical path is the TSDF weight recurrence, which a producer / consumer ring does not shorten; the warp-wide ray walk
-// costs more in rank searches than the scattered stores it saves) - kept as opt-in experiments.
 // The short-segment kernel is capped at short_ctas CTAs per SM through a dynamic shared-memory reservation so that a CTA of the
 // long-segment kernel (128 registers per thread) always finds room beside it - otherwise the two kernels run back to back.
 // short_t_ctas: the frame is bound by the long-segment kernel (128 registers per thread); whatever the short kernel takes from it
 // costs more than it gains.  Re-measured on an H100 80GB HBM3 (400 W, merged2, bench.py --quick, two alternating passes):
 // KSG_SHORT_T_CTAS 1 -> 164 frames/s, 2 -> 181-182, 3 -> 171-173, 4 -> 177-178; KSG_LONG_THREADS=128 172-176,
-// KSG_DEEP_THREADS=64 180-182, KSG_LONG_SERIAL=0 176-178 - the defaults below stay.
+// KSG_DEEP_THREADS=64 180-182 - the defaults below stay.  The non-hot long segments of C <= 32 run behind the short kernel, not
+// beside it: 181-182 against 176-178 frames/s in the same passes.
 struct Knobs {
   bool tile_apply = false;        // KSG_MERGED_TILE_APPLY=1: merged uses the tile kernel instead of the per-voxel kernels
-  bool short_thread = true;       // KSG_SHORT_THREAD=0: merged, C <= 32: the warp-per-voxel short kernel instead of k_voxel_apply_short_t
   int long_len = 0;               // KSG_LONG_LEN: records from which a voxel is long under k_voxel_apply_short_t (0: kLongLenThread)
-  bool l2_persist = false;        // KSG_L2_PERSIST=1: experiment, the (L * freq) rows persist in L2
-  bool hot_kernel = false;        // KSG_HOT_KERNEL=1
   int long_threads = 256;         // KSG_LONG_THREADS: 64, 128 or 256
   int long_grid = 0;              // KSG_LONG_GRID (0: one CTA per SM)
-  bool deep_hot = true;           // KSG_DEEP_HOT=0: the hot voxels do not get the deep-pipeline instance of k_voxel_apply_long
-  bool long_serial = true;        // KSG_LONG_SERIAL=0: the non-hot long segments (0.3 ms standalone) run beside the short kernel
   int deep_threads = 128;         // KSG_DEEP_THREADS: block size of the hot-voxel instance (32, 64, 128 or 256), one warp per chain
   int short_t_ctas = 2;           // KSG_SHORT_T_CTAS: CTAs per SM of k_voxel_apply_short_t, 1 to 8
   int short_ctas = 3;             // KSG_SHORT_CTAS: CTAs per SM of k_voxel_apply_short, 1 to 6
-  bool emit_warp = false;         // KSG_EMIT_WARP=1
   int solve_threads = kSolveThreads;   // KSG_SOLVE_THREADS: 256, 512 or 1024
   int solve_ctas_per_sm = INT_MAX;     // KSG_SOLVE_CTAS_PER_SM, at least 1 and at most what the occupancy allows
   bool profile_marks_only = false;     // KSG_PROFILE_MARKS_ONLY=1: fast, the solve kernel's phase marks without its per-ray probes
@@ -175,18 +167,12 @@ Knobs read_knobs() {
   auto env = [](const char* name, int* v) { const char* e = std::getenv(name); if (e) *v = std::atoi(e); return e != nullptr; };
   int v = 0;
   if (env("KSG_MERGED_TILE_APPLY", &v) && v != 0) k.tile_apply = true;
-  if (env("KSG_SHORT_THREAD", &v)) k.short_thread = v != 0;
   if (env("KSG_LONG_LEN", &v)) k.long_len = std::max(kLongLen, std::min(1 << 20, v));
-  if (env("KSG_L2_PERSIST", &v)) k.l2_persist = v != 0;
-  if (env("KSG_HOT_KERNEL", &v)) k.hot_kernel = v != 0;
   if (env("KSG_LONG_THREADS", &v) && (v == 64 || v == 128 || v == 256)) k.long_threads = v;
   if (env("KSG_LONG_GRID", &v)) k.long_grid = std::max(1, v);
-  if (env("KSG_DEEP_HOT", &v)) k.deep_hot = v != 0;
-  if (env("KSG_LONG_SERIAL", &v)) k.long_serial = v != 0;
   if (env("KSG_DEEP_THREADS", &v) && (v == 32 || v == 64 || v == 128 || v == 256)) k.deep_threads = v;
   if (env("KSG_SHORT_T_CTAS", &v)) k.short_t_ctas = std::max(1, std::min(8, v));
   if (env("KSG_SHORT_CTAS", &v)) k.short_ctas = std::max(1, std::min(6, v));
-  if (env("KSG_EMIT_WARP", &v)) k.emit_warp = v != 0;
   if (env("KSG_SOLVE_THREADS", &v) && (v == 256 || v == 512 || v == 1024)) k.solve_threads = v;
   if (env("KSG_SOLVE_CTAS_PER_SM", &v)) k.solve_ctas_per_sm = v;
   if (env("KSG_PROFILE_MARKS_ONLY", &v)) k.profile_marks_only = v != 0;
@@ -336,18 +322,12 @@ struct ksg_integrator {
   // merged, round-2 per-voxel apply (ksg_voxel.cuh)
   bool voxel_apply = false;
   VoxelQueues vq{};
-  cudaStream_t aux_stream = nullptr, aux_stream2 = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_join2 = nullptr;
-  // shape and experiments of the per-voxel kernels: development knobs (Knobs), set by ksg_create for the per-voxel apply only
-  bool hot_kernel = false;
-  bool emit_warp = false;
+  cudaStream_t aux_stream = nullptr;  // high priority, one kernel of the per-voxel apply per frame (merged_apply_voxels)
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  // shape of the per-voxel kernels: development knobs (Knobs), set by ksg_create for the per-voxel apply only
   int long_threads = 0, long_grid = 0, short_ctas = 0, short_smem = 0;
-  bool short_thread = false;         // merged, C <= 32: k_voxel_apply_short_t
-  bool long_serial = false;
   int deep_threads = 0;
-  bool deep_hot = false;             // merged, C <= 32: the hot voxels go to the deep-pipeline instance of k_voxel_apply_long
   int short_t_ctas = 0;
-  int hot_smem = 0;
 
   long long* tile_debug = nullptr;  // optional per-tile (records, cycles) trace
   int apply_smem = 0;
@@ -800,12 +780,8 @@ void merged_emit(ksg_integrator* h, MergedFrame& m) {
   ++h->n_launches;
   k_bundle_loglik<<<grid_for((long long)(nb + 1) * dc.C, B), B, 0, s>>>(dc, h->d_cnt, h->hist, h->tmp, h->tmp4);
   ++h->n_launches;
-  if (h->emit_warp)
-    k_emit_merged_warp<<<h->sm_count * 8, 256, 0, s>>>(dc, m.T, h->d_cnt, h->map, h->ray_param, h->ray_flags, h->b_key, h->nsteps, h->b_base,
-                                                       h->ks_sorted, m.cap, h->rec_a);
-  else
-    k_emit_merged<<<grid_for(nb, 128), 128, 0, s>>>(dc, m.T, h->d_cnt, h->map, h->ray_param, h->ray_flags, h->b_key, h->nsteps,
-                                                    h->b_base, h->ks_sorted, m.cap, h->rec_a);
+  k_emit_merged<<<grid_for(nb, 128), 128, 0, s>>>(dc, m.T, h->d_cnt, h->map, h->ray_param, h->ray_flags, h->b_key, h->nsteps,
+                                                  h->b_base, h->ks_sorted, m.cap, h->rec_a);
 }
 
 // The update records in (tile, voxel, order) order: per-voxel application order = reference order; then the frame's new blocks
@@ -825,7 +801,9 @@ int merged_sort_records(ksg_integrator* h, MergedFrame& m) {
   return KSG_OK;
 }
 
-// Per-voxel update (ksg_voxel.cuh): segment heads -> two queues; the long and the short kernel run concurrently
+// Per-voxel update (ksg_voxel.cuh): segment heads -> two queues; then one kernel on the high-priority side stream and the short
+// kernel on the frame's stream.  C <= 32: the hot voxels' chains (the DEEP instance, one warp per chain) beside the thread-per-voxel
+// short kernel, and the remaining long segments, little work, behind it.  C > 32: the long kernel beside the warp-per-voxel one.
 int merged_apply_voxels(ksg_integrator* h, MergedFrame& m) {
   const DevCfg& dc = h->dc;
   const Xform& T = m.T;
@@ -838,42 +816,21 @@ int merged_apply_voxels(ksg_integrator* h, MergedFrame& m) {
   const ApplySrc& src = m.src;
   KSG_CUDA(cudaEventRecord(h->ev_fork, s));
   KSG_CUDA(cudaStreamWaitEvent(h->aux_stream, h->ev_fork, 0));
-  // C <= 32: the voxels with thousands of records get one CTA each (third stream, concurrent with the other two kernels)
-  const int use_hot = (h->apply_nch == 1 && !h->hot_enabled && h->hot_kernel) ? 1 : 0;
-  bool deep_launched = false;
-  if (use_hot) {
-    KSG_CUDA(cudaStreamWaitEvent(h->aux_stream2, h->ev_fork, 0));
-    ++h->n_launches;
-    k_voxel_apply_hot<<<h->sm_count, 256, h->hot_smem, h->aux_stream2>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
-    KSG_CUDA(cudaEventRecord(h->ev_join2, h->aux_stream2));
-  }
-  h->n_launches += 2;
-  if (h->short_thread && h->apply_nch == 1) {
-    int skip = use_hot;
-    if (h->deep_hot && !use_hot) {   // the hot voxels' chains first, on their own high-priority stream (one warp per chain)
-      KSG_CUDA(cudaStreamWaitEvent(h->aux_stream2, h->ev_fork, 0));
-      ++h->n_launches;
-      k_voxel_apply_long<1, true><<<h->sm_count, h->deep_threads, 0, h->aux_stream2>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, 0);
-      KSG_CUDA(cudaEventRecord(h->ev_join2, h->aux_stream2));
-      skip = 1; deep_launched = true;
-    }
-    if (h->long_serial && deep_launched) {   // the remaining long segments are little work: behind the short kernel, on its stream
-      k_voxel_apply_short_t<<<h->sm_count * h->short_t_ctas, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
-      k_voxel_apply_long<1><<<h->long_grid, h->long_threads, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, skip);
-    } else {
-      k_voxel_apply_long<1><<<h->long_grid, h->long_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, skip);
-      k_voxel_apply_short_t<<<h->sm_count * h->short_t_ctas, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
-    }
+  if (h->apply_nch == 1) {
+    h->n_launches += 3;
+    k_voxel_apply_long<1, true><<<h->sm_count, h->deep_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, 0);
+    k_voxel_apply_short_t<<<h->sm_count * h->short_t_ctas, 256, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
+    k_voxel_apply_long<1><<<h->long_grid, h->long_threads, 0, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, 1);
   } else {
+    h->n_launches += 2;
     with_nch(h->apply_nch, [&](auto nch) {
       constexpr int NCH = decltype(nch)::value;
-      k_voxel_apply_long<NCH><<<h->long_grid, h->long_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, use_hot);
+      k_voxel_apply_long<NCH><<<h->long_grid, h->long_threads, 0, h->aux_stream>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq, 0);
       k_voxel_apply_short<NCH><<<h->sm_count * h->short_ctas, 256, h->short_smem, s>>>(dc, T, h->d_cnt, h->map, h->d_luts, h->rec_b, src, h->vq);
     });
   }
   KSG_CUDA(cudaEventRecord(h->ev_join, h->aux_stream));
   KSG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-  if (use_hot || deep_launched) KSG_CUDA(cudaStreamWaitEvent(s, h->ev_join2, 0));
   return KSG_OK;
 }
 
@@ -1253,12 +1210,9 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     if (h->voxel_apply) {
       h->vq.long_cap = 4 * (rec_cap / kLongLen) + 64;
       h->vq.long_len = kLongLen;
-      if (dc.C <= 32) {   // one thread per short voxel (ksg_voxel.cuh), unless KSG_SHORT_THREAD=0 selects the warp-per-voxel kernel
-        h->short_thread = knobs.short_thread;
-        if (h->short_thread) {
-          KSG_CUDA(res.device(&h->tmp4, (N + 1) * (size_t)((dc.C + 3) & ~3)));
-          h->vq.long_len = knobs.long_len ? knobs.long_len : kLongLenThread;
-        }
+      if (dc.C <= 32) {   // one thread per short voxel (ksg_voxel.cuh)
+        KSG_CUDA(res.device(&h->tmp4, (N + 1) * (size_t)((dc.C + 3) & ~3)));
+        h->vq.long_len = knobs.long_len ? knobs.long_len : kLongLenThread;
       }
       h->vq.short_cap = rec_cap;
       KSG_CUDA(res.device(&h->vq.long_items, (size_t)h->vq.long_cap));
@@ -1270,36 +1224,8 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
       }
       KSG_CUDA(res.event(&h->ev_fork, cudaEventDisableTiming));
       KSG_CUDA(res.event(&h->ev_join, cudaEventDisableTiming));
-      {
-        int lo_p = 0, hi_p = 0;
-        KSG_CUDA(cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
-        KSG_CUDA(res.stream(&h->aux_stream2, hi_p));
-      }
-      KSG_CUDA(res.event(&h->ev_join2, cudaEventDisableTiming));
-      if (knobs.l2_persist) {
-        // experiment: keep the (L * freq) rows resident in L2 while the update kernels stream records and voxel data through it
-        cudaDeviceProp prop{};
-        KSG_CUDA(cudaGetDeviceProperties(&prop, h->device));
-        const size_t want = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, 32u << 20);
-        if (want > 0) {
-          KSG_CUDA(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want));
-          cudaStreamAttrValue attr{};
-          attr.accessPolicyWindow.base_ptr = h->tmp;
-          attr.accessPolicyWindow.num_bytes = std::min<size_t>((size_t)(N + 1) * dc.C * sizeof(float), (size_t)prop.accessPolicyMaxWindowSize);
-          attr.accessPolicyWindow.hitRatio = 1.0f;
-          attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-          attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-          KSG_CUDA(cudaStreamSetAttribute(h->aux_stream2, cudaStreamAttributeAccessPolicyWindow, &attr));
-          KSG_CUDA(cudaStreamSetAttribute(h->aux_stream, cudaStreamAttributeAccessPolicyWindow, &attr));
-        }
-      }
-      h->hot_smem = 2 * kHotChunkRecs * (32 * (int)sizeof(float) + (int)sizeof(float4));
-      KSG_CUDA(cudaFuncSetAttribute(k_voxel_apply_hot, cudaFuncAttributeMaxDynamicSharedMemorySize, h->hot_smem));
-      h->hot_kernel = knobs.hot_kernel;
       h->long_threads = knobs.long_threads;
       h->long_grid = knobs.long_grid ? knobs.long_grid : h->sm_count;
-      h->deep_hot = knobs.deep_hot;
-      h->long_serial = knobs.long_serial;
       h->deep_threads = knobs.deep_threads;
       h->short_t_ctas = knobs.short_t_ctas;
       h->short_ctas = knobs.short_ctas;
@@ -1311,7 +1237,6 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
         });
         if (rc) return rc;
       }
-      h->emit_warp = knobs.emit_warp;
     }
     if (cfg->hot_voxel_mode >= 1 && dc.C <= 32 && cfg->apply_mode == 0) {
       h->hot_enabled = true;

@@ -30,9 +30,9 @@ HOT_LEN = 4096              # kHotLen
 TRACK_LEN = 32              # voxels with at least one full batch are followed through the branch model
 
 
-def long_len(num_labels, short_thread=True, env_long_len=None):
+def long_len(num_labels, env_long_len=None):
     """ksg_create: segments of at least this many records are `long` (thread-per-voxel short kernel at C <= 32, else warp-per-voxel)."""
-    if num_labels <= 32 and short_thread:
+    if num_labels <= 32:
         return 256 if env_long_len is None else max(96, min(1 << 20, env_long_len))
     return 96
 

@@ -20,8 +20,7 @@ SUBSET = ("route_edge_n256_c21", "route_edge_n4095_c21", "route_edge_n4096_c21",
           "class_count_merged_c33")
 CFG_VARIANTS = {"apply_mode_1": {"apply_mode": 1}, "hot_voxel_mode_1": {"hot_voxel_mode": 1}, "hot_voxel_mode_2": {"hot_voxel_mode": 2},
                 "libstdcxx_bundle_order": {"merged_bundle_order": 1}}
-ENV_VARIANTS = {"KSG_SHORT_THREAD": 0, "KSG_DEEP_HOT": 0, "KSG_HOT_KERNEL": 1, "KSG_LONG_SERIAL": 0, "KSG_MERGED_TILE_APPLY": 1,
-                "KSG_LONG_LEN": 4096}
+ENV_VARIANTS = {"KSG_MERGED_TILE_APPLY": 1, "KSG_LONG_LEN": 4096}
 
 
 def oracle_frames(cfg, frames):
@@ -93,7 +92,7 @@ def expected_routes(cfg, cert, env):
     import apply_edge_scenes as S
     if cfg.apply_mode == 1 or int(env.get("KSG_MERGED_TILE_APPLY", 0)) != 0:
         return [{"hot": 0, "long": 0, "short": 0} for _ in cert]            # the tile kernel: no queues
-    llen = S.long_len(cfg.num_labels, short_thread=int(env.get("KSG_SHORT_THREAD", 1)) != 0, env_long_len=env.get("KSG_LONG_LEN"))
+    llen = S.long_len(cfg.num_labels, env_long_len=env.get("KSG_LONG_LEN"))
     return [S.routes(c["lengths"], llen) for c in cert]
 
 

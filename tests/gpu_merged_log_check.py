@@ -19,8 +19,7 @@ sys.path.insert(0, HERE)
 SCENES = ("route_edge_n255_c21", "route_edge_n256_c21", "route_edge_n4095_c21", "route_edge_n4096_c21", "route_edge_n4160_c21",
           "route_edge_n96_c33", "weight_states_default", "moving_distance_semantic", "class_count_merged_c33")
 CFG_VARIANTS = {"apply_mode_1": {"apply_mode": 1}, "hot_voxel_mode_1": {"hot_voxel_mode": 1}, "hot_voxel_mode_2": {"hot_voxel_mode": 2}}
-ENV_VARIANTS = {"KSG_SHORT_THREAD": 0, "KSG_DEEP_HOT": 0, "KSG_HOT_KERNEL": 1, "KSG_LONG_SERIAL": 0, "KSG_MERGED_TILE_APPLY": 1,
-                "KSG_LONG_LEN": 4096}
+ENV_VARIANTS = {"KSG_MERGED_TILE_APPLY": 1, "KSG_LONG_LEN": 4096}
 
 
 def values_match(heads, pri, exp):

@@ -4,10 +4,10 @@ that start at zero, cross the clamp inside a batch and start saturated, distance
 counts at the kernel switches.  tests/test_apply_edge_scenes_cpu.py proves on the CPU which paths each scene takes.
 
 Every frame of every scene is compared with the oracle bit for bit (counters, every exported field, updated() blocks), under the
-default routes and again under each in-tree alternative: KSG_SHORT_THREAD=0, KSG_DEEP_HOT=0, KSG_HOT_KERNEL=1, KSG_LONG_SERIAL=0,
-KSG_MERGED_TILE_APPLY=1, KSG_LONG_LEN=4096 (each set only around the creation of the one integrator it is for, in a helper process
-that starts without them), apply_mode 1, hot_voxel_mode 1 and 2 and the reference's bundle order.  The voxels the device queued per
-route (ksg_debug_apply_routes) must equal the certificate's counts, and hot_voxel_mode 2 must actually skip the saturated camera voxel."""
+default routes and again under each in-tree alternative: KSG_MERGED_TILE_APPLY=1, KSG_LONG_LEN=4096 (each set only around the
+creation of the one integrator it is for, in a helper process that starts without them), apply_mode 1, hot_voxel_mode 1 and 2 and
+the reference's bundle order.  The voxels the device queued per route (ksg_debug_apply_routes) must equal the certificate's counts,
+and hot_voxel_mode 2 must actually skip the saturated camera voxel."""
 import json
 import os
 import subprocess

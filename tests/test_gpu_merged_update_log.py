@@ -121,17 +121,19 @@ def route_report():
 
 
 def test_the_log_is_the_same_bytes_under_every_apply_route_and_on_every_run(route_report):
-    """The scenes with hot voxels and segments on the route thresholds: the log bytes under KSG_SHORT_THREAD=0, KSG_DEEP_HOT=0,
-    KSG_HOT_KERNEL=1, KSG_LONG_SERIAL=0, KSG_MERGED_TILE_APPLY=1, KSG_LONG_LEN=4096, apply_mode 1 and hot_voxel_mode 1 / 2, and from a
-    second integrator, equal those of the default routes; frame 0 logs the traced voxels with the exported state."""
-    from gpu_merged_log_check import SCENES
+    """The scenes with hot voxels and segments on the route thresholds: the log bytes under KSG_MERGED_TILE_APPLY=1,
+    KSG_LONG_LEN=4096, apply_mode 1 and hot_voxel_mode 1 / 2, and from a second integrator, equal those of the default routes;
+    frame 0 logs the traced voxels with the exported state."""
+    from gpu_merged_log_check import CFG_VARIANTS, ENV_VARIANTS, SCENES
     assert set(route_report) == set(SCENES)
     for name, r in route_report.items():
         assert not r["failures"], (name, r["failures"])
         base = r["runs"]["default"]
         assert all(f[0] > 0 for f in base), name
         assert all(f[4] for v in r["runs"].values() for f in v), (name, "log entries differ from the exported map")
-        assert len(r["runs"]) >= 8, name
+        configs = {"default", "default_again"} | {f"{k}={v}" for k, v in ENV_VARIANTS.items()}
+        configs |= {k for k in CFG_VARIANTS if not (k.startswith("hot_voxel") and name.endswith("_c33"))}
+        assert set(r["runs"]) == configs, name
         bad = {k: [(f, v[f][3] != base[f][3]) for f in range(len(v)) if v[f] != base[f]] for k, v in r["runs"].items() if v != base}
         assert not bad, (name, "configuration: [(frame, the exported map differs too)]", bad)
 
