@@ -351,6 +351,34 @@ int32_t ksg_query_points(ksg_integrator* h, int64_t n, const float* xyz_G, float
 int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, float min_weight, const ksg_query_out* d_out,
                                 void* cuda_stream);
 
+/* Depth and semantic images of the device map from a camera pose: per pixel, a ray march to the first zero crossing of the trilinear
+ * TSDF distance (the one ksg_query_points returns), then the point query at the hit.  A new capability, not part of the reference:
+ * unpinned; csrc/ksg_render.cuh states every rule.  T_G_C: 7 floats (qw qx qy qz tx ty tz) as for the depth entries; K = fx fy cx cy;
+ * pixel (u, v) is index v * width + u and its ray is the one ksg_integrate_depth_k64 back-projects, so a render at an integration pose
+ * walks exactly the rays that frame integrated.  The march starts at camera depth min_depth and gives up past max_depth:
+ *   - depth: camera-frame z of the hit; points_G: the world-frame hit point; NaN (both) on a miss;
+ *   - at_hit: ksg_query_points(points_G, min_weight) - the containing voxel with its semantic row, the trilinear distance and its
+ *     gradient (normal = gradient / |gradient|); a miss gets the answer for a NaN point (flags 0, NaN, 0 bytes).
+ * Every pointer may be NULL (= not wanted) and an unwanted array is never written.  Rejected (KSG_ERR_INVALID_ARGUMENT): a NULL handle,
+ * pose, K or out; a non-finite pose or K; fx or fy <= 0; width or height <= 0; min_depth not finite or <= 0; max_depth not finite or
+ * <= min_depth; a NaN or negative min_weight; a spatially sharded integrator (as ksg_query_points); and the step-rounding rule:
+ *     (voxel_size / 4) / r_max < max_depth * 2^-20,   r_max = |((u - cx) / fx, (v - cy) / fy, 1)| at the image corner farthest from (cx, cy)
+ * (the march's smallest z step would come within 8 ulp of z, which could stall it).  Nothing wanted returns KSG_OK without touching the
+ * device (the host entry still completes the pending frame); depth and / or points_G alone is one kernel launch, any at_hit output two.
+ * ksg_render_view: host buffers; completes the pending frame, stages through one temporary device buffer, returns when done.
+ * ksg_render_view_device: the arrays of *d_out are DEVICE memory (the struct and the pose / K are read on the host during the call); it
+ * only enqueues on `cuda_stream` (NULL = the integrator's own stream), with the stream order and ownership of ksg_query_points_device.
+ * Any at_hit output needs points_G (the query reads the hit points from it; rejected otherwise). */
+typedef struct ksg_render_out {
+  float* depth;            /* W*H, camera-frame z of the hit, NaN on a miss */
+  float* points_G;         /* 3*W*H, world-frame hit point, NaN on a miss */
+  ksg_query_out at_hit;    /* ksg_query_points at points_G; every pointer may be NULL */
+} ksg_render_out;
+int32_t ksg_render_view(ksg_integrator* h, const float* T_G_C, const double* K, int32_t width, int32_t height,
+                        float min_depth, float max_depth, float min_weight, const ksg_render_out* out);
+int32_t ksg_render_view_device(ksg_integrator* h, const float* T_G_C_host, const double* K_host, int32_t width, int32_t height,
+                               float min_depth, float max_depth, float min_weight, const ksg_render_out* d_out, void* cuda_stream);
+
 /* Remove every block but keep the integrator: what Layer::removeAllBlocks() on both layers does to a live reference integrator.  The
  * fast integrator's two per-scan approximate sets (members of the integrator, fast.h:114-130) keep their contents and offsets, so the
  * next frame is integrated exactly as the reference integrator object would integrate it into its emptied layers.  Used by the

@@ -102,6 +102,21 @@ class KsgQueryOut(C.Structure):
     _fields_ = [(name, C.c_void_p) for name in QUERY_FIELDS]
 
 
+RENDER_FIELDS = ("depth", "points_G") + QUERY_FIELDS
+
+
+class KsgRenderOut(C.Structure):
+    """Mirror of `struct ksg_render_out` (include/ksg.h): depth, points_G, then the point query at the hit (at_hit); NULL = not wanted."""
+    _fields_ = [("depth", C.c_void_p), ("points_G", C.c_void_p), ("at_hit", KsgQueryOut)]
+
+    @classmethod
+    def of(cls, ptrs: Dict[str, int]) -> "KsgRenderOut":
+        """from a {field of RENDER_FIELDS: address} dict; missing or 0 = not wanted"""
+        ptrs = {k: int(v) for k, v in ptrs.items() if v}
+        return cls(depth=ptrs.get("depth"), points_G=ptrs.get("points_G"),
+                   at_hit=KsgQueryOut(**{k: v for k, v in ptrs.items() if k in QUERY_FIELDS}))
+
+
 def label_palette(num_labels: int) -> np.ndarray:
     """A deterministic label -> RGBA table (label 0 = white as color.cpp:64-66 forces)."""
     pal = np.zeros((256, 4), dtype=np.uint8)
@@ -270,6 +285,11 @@ def load_library(path: Optional[str] = None):
     lib.ksg_query_points.restype = C.c_int32
     lib.ksg_query_points_device.argtypes = [H, C.c_int64, C.c_void_p, C.c_float, C.POINTER(KsgQueryOut), C.c_void_p]
     lib.ksg_query_points_device.restype = C.c_int32
+    lib.ksg_render_view.argtypes = [H, fp, dp, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float, C.POINTER(KsgRenderOut)]
+    lib.ksg_render_view.restype = C.c_int32
+    lib.ksg_render_view_device.argtypes = [H, fp, dp, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float, C.POINTER(KsgRenderOut),
+                                           C.c_void_p]
+    lib.ksg_render_view_device.restype = C.c_int32
     lib.ksg_clear_map.argtypes = [H]
     lib.ksg_clear_map.restype = C.c_int32
     lib.ksg_build_info.argtypes = []
@@ -286,7 +306,7 @@ KSG_SYMBOLS = ["ksg_default_config", "ksg_create", "ksg_destroy", "ksg_last_erro
                "ksg_unordered_map_schedule", "ksg_integrate_depth_k64", "ksg_integrate_depth_device_k64",
                "ksg_debug_chain_sum", "ksg_debug_tsdf_batch", "ksg_debug_apply_routes", "ksg_debug_fast_timeline", "ksg_integrate_depth_async", "ksg_wait_frame",
                "ksg_device_map_view", "ksg_merge_blocks_device", "ksg_copy_map_device", "ksg_integrate_image", "ksg_set_update_log", "ksg_fetch_update_log", "ksg_evaluate_labels", "ksg_extract_mesh", "ksg_clear_map", "ksg_copy_update_log_device", "ksg_merge_voxels_device",
-               "ksg_query_points", "ksg_query_points_device"]
+               "ksg_query_points", "ksg_query_points_device", "ksg_render_view", "ksg_render_view_device"]
 
 
 def debug_chain_sum(terms: np.ndarray, s0: float, lib=None) -> np.float32:
@@ -652,6 +672,32 @@ class Integrator:
         q = KsgQueryOut(**{k: int(v) for k, v in out_ptrs.items() if v})
         self._check(self.lib.ksg_query_points_device(self.handle, n, C.c_void_p(d_xyz), min_weight, C.byref(q), C.c_void_p(stream)),
                     "ksg_query_points_device")
+
+    def render(self, T_G_C, K, width: int, height: int, min_depth: float, max_depth: float, min_weight: float = 1e-4,
+               fields=RENDER_FIELDS) -> Dict[str, np.ndarray]:
+        """Depth and semantic images of the device map from pose T_G_C (ksg_render_view; K = fx fy cx cy, float64): a dict of the
+        wanted `fields` (of RENDER_FIELDS) as [H, W, ...] arrays - depth [H, W] f32 (camera z of the hit, NaN on a miss), points_G
+        [H, W, 3] f32, and the point query at the hit (the keys, dtypes and trailing shapes of query_points)."""
+        T = np.ascontiguousarray(T_G_C, np.float32)
+        Kd = np.ascontiguousarray(K, np.float64)
+        shape = {"depth": (), "points_G": (3,), "flags": (), "tsdf_distance": (), "tsdf_weight": (), "tsdf_rgba": (4,), "sem_label": (),
+                 "sem_priors": (self.cfg.num_labels,), "sem_rgba": (4,), "distance": (), "gradient": (3,)}
+        u8 = ("flags", "tsdf_rgba", "sem_label", "sem_rgba")
+        out = {k: np.zeros((height, width) + shape[k], np.uint8 if k in u8 else np.float32) for k in fields}
+        o = KsgRenderOut.of({k: v.ctypes.data for k, v in out.items()})
+        self._check(self.lib.ksg_render_view(self.handle, _ptr(T, C.c_float), _ptr(Kd, C.c_double), width, height, min_depth, max_depth,
+                                             min_weight, C.byref(o)), "ksg_render_view")
+        return out
+
+    def render_device(self, T_G_C, K, width: int, height: int, min_depth: float, max_depth: float, out_ptrs: Dict[str, int],
+                      stream: int = 0, min_weight: float = 1e-4):
+        """Enqueue ksg_render_view_device on `stream` (0 = the integrator's own stream): the values of out_ptrs (keys of RENDER_FIELDS;
+        missing keys = not wanted) are raw device pointers; any query field needs points_G.  Returns without waiting."""
+        T = np.ascontiguousarray(T_G_C, np.float32)
+        Kd = np.ascontiguousarray(K, np.float64)
+        o = KsgRenderOut.of(out_ptrs)
+        self._check(self.lib.ksg_render_view_device(self.handle, _ptr(T, C.c_float), _ptr(Kd, C.c_double), width, height, min_depth,
+                                                    max_depth, min_weight, C.byref(o), C.c_void_p(stream)), "ksg_render_view_device")
 
     def last_updated_blocks(self) -> np.ndarray:
         n = int(self.lib.ksg_last_updated_blocks(self.handle, 0, None))

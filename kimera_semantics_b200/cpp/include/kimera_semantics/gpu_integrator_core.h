@@ -48,6 +48,16 @@ class GpuIntegratorCore {
     std::vector<float> distance, gradient;            // n, 3n
   };
   bool queryPoints(const vxb::Pointcloud& points_G, float min_weight, QueryResult* result);
+  // Depth and semantic images of the device map from pose T_G_C (ksg_render_view), read-only like queryPoints: works in kLazy mode
+  // without syncLayers().  K = fx fy cx cy.  Per pixel (row-major, w * h): the camera depth and world point of the first surface hit
+  // (NaN on a miss) and queryPoints' answer at that point.
+  struct RenderResult {
+    std::vector<float> depth;      // w * h
+    std::vector<float> points_G;   // 3 * w * h
+    QueryResult at_hit;            // w * h points
+  };
+  bool renderView(const vxb::Transformation& T_G_C, const double K[4], int w, int h, float min_depth, float max_depth, float min_weight,
+                  RenderResult* result);
   int64_t lastVoxelUpdates() const { return last_voxel_updates_; }
   ksg_integrator* handle() { return handle_; }
 

@@ -107,6 +107,13 @@ class SemanticTsdfServer {
     return gpu().queryPoints(points_G, min_weight, result);
   }
 
+  // What a camera at T_G_C would see of the fused map - depth, hit points, labels, normals (gradient) - rendered on the device from the
+  // device map (ksg_render_view, csrc/ksg_render.cuh): needs no updateLayers().
+  bool renderView(const vxb::Transformation& T_G_C, const double K[4], int w, int h, float min_depth, float max_depth, float min_weight,
+                  GpuIntegratorCore::RenderResult* result) {
+    return gpu().renderView(T_G_C, K, w, h, min_depth, max_depth, min_weight, result);
+  }
+
   vxb::Layer<vxb::TsdfVoxel>* getTsdfLayerPtr() { return tsdf_layer_.get(); }
   vxb::Layer<SemanticVoxel>* getSemanticLayerPtr() { return semantic_layer_.get(); }
   vxb::TsdfIntegratorBase* getIntegratorPtr() { return tsdf_integrator_.get(); }

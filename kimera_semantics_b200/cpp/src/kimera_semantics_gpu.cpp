@@ -324,6 +324,30 @@ bool GpuIntegratorCore::queryPoints(const vxb::Pointcloud& points_G, float min_w
   return ksg_query_points(handle_, (int64_t)n, n ? reinterpret_cast<const float*>(points_G.data()) : nullptr, min_weight, &out) == KSG_OK;
 }
 
+bool GpuIntegratorCore::renderView(const vxb::Transformation& T_G_C, const double K[4], int w, int h, float min_depth, float max_depth,
+                                   float min_weight, RenderResult* r) {
+  const vxb::FloatingPoint* q = T_G_C.getRotationWxyz();
+  const vxb::Point& t = T_G_C.getPosition();
+  const float T[7] = {q[0], q[1], q[2], q[3], t.x(), t.y(), t.z()};
+  const size_t n = (w > 0 && h > 0) ? (size_t)w * (size_t)h : 0;
+  QueryResult& a = r->at_hit;
+  r->depth.assign(n, 0.0f);
+  r->points_G.assign(3 * n, 0.0f);
+  a.flags.assign(n, 0);
+  a.tsdf_distance.assign(n, 0.0f);
+  a.tsdf_weight.assign(n, 0.0f);
+  a.tsdf_rgba.assign(4 * n, 0);
+  a.sem_label.assign(n, 0);
+  a.sem_priors.assign(n * kTotalNumberOfLabels, 0.0f);
+  a.sem_rgba.assign(4 * n, 0);
+  a.distance.assign(n, 0.0f);
+  a.gradient.assign(3 * n, 0.0f);
+  ksg_render_out out = {r->depth.data(), r->points_G.data(),
+                        {a.flags.data(), a.tsdf_distance.data(), a.tsdf_weight.data(), a.tsdf_rgba.data(), a.sem_label.data(),
+                         a.sem_priors.data(), a.sem_rgba.data(), a.distance.data(), a.gradient.data()}};
+  return ksg_render_view(handle_, T, K, w, h, min_depth, max_depth, min_weight, &out) == KSG_OK;
+}
+
 void GpuIntegratorCore::uploadLayers() {
   vxb::BlockIndexList blocks;
   tsdf_layer_->getAllAllocatedBlocks(&blocks);

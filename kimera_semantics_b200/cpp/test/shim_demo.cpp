@@ -1,6 +1,6 @@
 // Drives the drop-in C++ API exactly the way SemanticTsdfServer does (kimera_semantics_ros/src/semantic_tsdf_server.cpp:58-79):
 // build both layers, SemanticTsdfIntegratorFactory::create(method, ...), then integratePointCloud per frame.
-//   shim_demo <fast|merged|bogus> <frames.bin> <out.bin> [lazy] [--load ckpt] [--save ckpt] [--skip N] [--query in out]
+//   shim_demo <fast|merged|bogus> <frames.bin> <out.bin> [lazy] [--load ckpt] [--save ckpt] [--skip N] [--query in out] [--render in out]
 //     --load: SemanticTsdfServer::loadMap before the first frame; --save: saveMap after the last; --skip: ignore the first N frames
 //     --depth file: instead of the clouds of frames.bin (whose frame count must then be 0) feed depth + label frames:
 //              int32 n, int32 width, int32 height, double K[4], then per frame float T[7], float depth[w*h], uint8 label[w*h]
@@ -8,6 +8,9 @@
 //              `in` (int32 n, float xyz[3n], world frame; min_weight 1e-4); `out` = the arrays of QueryResult one after the other:
 //              flags[n] u8, tsdf_distance[n] f32, tsdf_weight[n] f32, tsdf_rgba[4n] u8, sem_label[n] u8, sem_priors[n*C] f32,
 //              sem_rgba[4n] u8, distance[n] f32, gradient[3n] f32
+//     --render in out: after the last frame (also before any layer sync) SemanticTsdfServer::renderView with `in` = float T_G_C[7],
+//              double K[4], int32 w, int32 h, float min_depth, max_depth, min_weight; `out` = depth[n] f32, points_G[3n] f32, then the
+//              arrays of --query's output for the n = w * h hit points
 // frames.bin : int32 n_frames, float voxel_size, int32 vps, int32 n_palette, palette n*(r,g,b,a,id), int32 n_dynamic, ids...,
 //              then per frame: int32 n, float T[7], float xyz[3n], uint8 rgba[4n]
 // out.bin    : int32 n_blocks, then per block (sorted z,y,x): int32 idx[3], per voxel: float d, float w, u8 rgba[4], u8 label,
@@ -45,6 +48,7 @@ int main(int argc, char** argv) {
   config.default_truncation_distance = 4.0f * voxel_size;  // voxblox_ros
   bool lazy = false;
   const char *load_path = nullptr, *save_path = nullptr, *depth_path = nullptr, *query_in = nullptr, *query_out = nullptr;
+  const char *render_in = nullptr, *render_out = nullptr;
   int skip = 0;
   for (int a = 4; a < argc; ++a) {
     if (std::strcmp(argv[a], "lazy") == 0) lazy = true;
@@ -53,6 +57,7 @@ int main(int argc, char** argv) {
     else if (std::strcmp(argv[a], "--skip") == 0 && a + 1 < argc) skip = std::atoi(argv[++a]);
     else if (std::strcmp(argv[a], "--depth") == 0 && a + 1 < argc) depth_path = argv[++a];
     else if (std::strcmp(argv[a], "--query") == 0 && a + 2 < argc) { query_in = argv[++a]; query_out = argv[++a]; }
+    else if (std::strcmp(argv[a], "--render") == 0 && a + 2 < argc) { render_in = argv[++a]; render_out = argv[++a]; }
   }
   SemanticTsdfServer::Params params;
   params.tsdf_voxel_size = voxel_size;
@@ -115,6 +120,37 @@ int main(int argc, char** argv) {
     size_t hits = 0;
     for (uint8_t fl : q.flags) hits += (fl & KSG_QUERY_OBSERVED) ? 1 : 0;
     std::printf("point query: %d points, %zu in observed voxels%s\n", n, hits, lazy ? " (host layers not synchronised)" : "");
+  }
+  if (render_in) {
+    std::ifstream rf(render_in, std::ios::binary);
+    KSG_CHECK(rf.good()) << "cannot open " << render_in;
+    float T[7];
+    double K[4];
+    rf.read(reinterpret_cast<char*>(T), sizeof(T));
+    rf.read(reinterpret_cast<char*>(K), sizeof(K));
+    const int w = rd<int32_t>(rf), h = rd<int32_t>(rf);
+    float depth_range[3];
+    rf.read(reinterpret_cast<char*>(depth_range), sizeof(depth_range));
+    GpuIntegratorCore::RenderResult rr;
+    KSG_CHECK(server.renderView(vxb::Transformation(T[0], T[1], T[2], T[3], vxb::Point(T[4], T[5], T[6])), K, w, h, depth_range[0],
+                                depth_range[1], depth_range[2], &rr)) << "render failed";
+    std::ofstream ro(render_out, std::ios::binary);
+    auto put = [&ro](const void* p, size_t bytes) { ro.write(reinterpret_cast<const char*>(p), bytes); };
+    const GpuIntegratorCore::QueryResult& q = rr.at_hit;
+    put(rr.depth.data(), 4 * rr.depth.size());
+    put(rr.points_G.data(), 4 * rr.points_G.size());
+    put(q.flags.data(), q.flags.size());
+    put(q.tsdf_distance.data(), 4 * q.tsdf_distance.size());
+    put(q.tsdf_weight.data(), 4 * q.tsdf_weight.size());
+    put(q.tsdf_rgba.data(), q.tsdf_rgba.size());
+    put(q.sem_label.data(), q.sem_label.size());
+    put(q.sem_priors.data(), 4 * q.sem_priors.size());
+    put(q.sem_rgba.data(), q.sem_rgba.size());
+    put(q.distance.data(), 4 * q.distance.size());
+    put(q.gradient.data(), 4 * q.gradient.size());
+    size_t hits = 0;
+    for (float d : rr.depth) hits += (d == d) ? 1 : 0;
+    std::printf("render: %dx%d pixels, %zu hits%s\n", w, h, hits, lazy ? " (host layers not synchronised)" : "");
   }
   if (lazy) server.updateLayers();
   {

@@ -30,6 +30,7 @@
 #include "ksg_eval.cuh"
 #include "ksg_mesh.cuh"
 #include "ksg_query.cuh"
+#include "ksg_render.cuh"
 
 using namespace ksg;
 
@@ -1875,6 +1876,101 @@ int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz
   if (!work) return KSG_OK;
   KSG_CUDA(cudaSetDevice(h->device));
   launch_query(h, n, d_xyz_G, min_weight, *d_out, cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream);
+  KSG_CUDA(cudaGetLastError());
+  return KSG_OK;
+}
+
+namespace {
+bool query_wanted(const ksg_query_out& o) {
+  return o.flags || o.tsdf_distance || o.tsdf_weight || o.tsdf_rgba || o.sem_label || o.sem_priors || o.sem_rgba || o.distance || o.gradient;
+}
+// the checks both render entries share; fills the kernel's camera
+int render_args(ksg_integrator* h, const float* T, const double* K, int32_t width, int32_t height, float min_depth, float max_depth,
+                float min_weight, const ksg_render_out* o, RenderCam* c) {
+  if (!h) return KSG_ERR_INVALID_ARGUMENT;
+  if (!T || !K || !o) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: NULL pose, K or out");
+  for (int k = 0; k < 7; ++k)
+    if (!std::isfinite(T[k])) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: non-finite pose");
+  for (int k = 0; k < 4; ++k)
+    if (!std::isfinite(K[k])) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: non-finite K");
+  if (!(K[0] > 0.0) || !(K[1] > 0.0)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: fx or fy <= 0");
+  if (width <= 0 || height <= 0) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: width or height <= 0");
+  if (!std::isfinite(min_depth) || !(min_depth > 0.0f) || !std::isfinite(max_depth) || !(max_depth > min_depth))
+    return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: needs 0 < min_depth < max_depth, both finite");
+  if (!(min_weight >= 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: NaN or negative min_weight");
+  // the smallest z step, (kRenderPush * vs) / r at the corner pixel with the largest r, must be >= max_depth * 2^-20 (ksg_render.cuh)
+  const double au = std::max(std::fabs(0.0 - K[2]), std::fabs((double)(width - 1) - K[2])) / K[0];
+  const double av = std::max(std::fabs(0.0 - K[3]), std::fabs((double)(height - 1) - K[3])) / K[1];
+  const double r_max = std::sqrt(au * au + av * av + 1.0);
+  if (!((double)kRenderPush * (double)h->dc.voxel_size / r_max >= (double)max_depth * 0x1p-20))
+    return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: max_depth too large for the voxel size and field of view (a step would round away)");
+  if (h->dc.shard_count > 1) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: a sharded integrator holds only its own tiles");
+  c->T = Xform{T[0], T[1], T[2], T[3], T[4], T[5], T[6]};
+  c->cx = (float)K[2];
+  c->cy = (float)K[3];
+  c->constant_x = (float)(1.0 / K[0]);
+  c->constant_y = (float)(1.0 / K[1]);
+  c->width = width;
+  c->height = height;
+  c->min_depth = min_depth;
+  c->max_depth = max_depth;
+  c->min_weight = min_weight;
+  return KSG_OK;
+}
+// the march (writes depth and / or points), then the point query at the points when an at_hit output is wanted
+void launch_render(ksg_integrator* h, const RenderCam& c, float* d_depth, float* d_points, const ksg_query_out& at_hit, cudaStream_t s) {
+  const int64_t tiles = (int64_t)((c.width + kRenderTileW - 1) / kRenderTileW) * ((c.height + kRenderTileH - 1) / kRenderTileH);
+  const int grid = (int)((tiles * 32 + kRenderThreads - 1) / kRenderThreads);
+  ++h->n_launches;
+  k_render_view<<<grid, kRenderThreads, 0, s>>>(h->dc, h->map, c, d_depth, d_points);
+  if (query_wanted(at_hit)) launch_query(h, (int64_t)c.width * c.height, d_points, c.min_weight, at_hit, s);
+}
+}  // namespace
+
+int32_t ksg_render_view(ksg_integrator* h, const float* T_G_C, const double* K, int32_t width, int32_t height, float min_depth,
+                        float max_depth, float min_weight, const ksg_render_out* out) {
+  RenderCam c{};
+  { const int rca = render_args(h, T_G_C, K, width, height, min_depth, max_depth, min_weight, out, &c); if (rca) return rca; }
+  KSG_CUDA(cudaSetDevice(h->device));
+  KSG_CUDA(cudaDeviceSynchronize());
+  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  const ksg_query_out& o = out->at_hit;
+  const bool at_hit = query_wanted(o);
+  if (!out->depth && !out->points_G && !at_hit) return KSG_OK;
+  const size_t N = (size_t)width * (size_t)height, C = (size_t)h->dc.C;
+  // one device buffer: depth, points (also when only at_hit outputs are wanted: the query reads them), then every wanted query output
+  const size_t sizes[11] = {out->depth ? 4 * N : 0, (out->points_G || at_hit) ? 12 * N : 0, o.flags ? N : 0, o.tsdf_distance ? 4 * N : 0,
+                            o.tsdf_weight ? 4 * N : 0, o.tsdf_rgba ? 4 * N : 0, o.sem_label ? N : 0, o.sem_priors ? 4 * N * C : 0,
+                            o.sem_rgba ? 4 * N : 0, o.distance ? 4 * N : 0, o.gradient ? 12 * N : 0};
+  size_t off[11], total = 0;
+  for (int k = 0; k < 11; ++k) { off[k] = total; total += (sizes[k] + 255) / 256 * 256; }
+  Resources tmp;
+  uint8_t* d = nullptr;
+  KSG_CUDA(tmp.device(&d, total));
+  auto at = [&](int k) -> void* { return sizes[k] ? (void*)(d + off[k]) : nullptr; };
+  ksg_query_out dq{(uint8_t*)at(2), (float*)at(3), (float*)at(4), (uint8_t*)at(5), (uint8_t*)at(6), (float*)at(7), (uint8_t*)at(8),
+                   (float*)at(9), (float*)at(10)};
+  void* host[11] = {out->depth, out->points_G, o.flags, o.tsdf_distance, o.tsdf_weight, o.tsdf_rgba, o.sem_label, o.sem_priors, o.sem_rgba,
+                    o.distance, o.gradient};
+  cudaStream_t s = h->own_stream;
+  launch_render(h, c, (float*)at(0), (float*)at(1), dq, s);
+  KSG_CUDA(cudaGetLastError());
+  for (int k = 0; k < 11; ++k)
+    if (host[k]) KSG_CUDA(cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
+  return KSG_OK;
+}
+
+int32_t ksg_render_view_device(ksg_integrator* h, const float* T_G_C_host, const double* K_host, int32_t width, int32_t height,
+                               float min_depth, float max_depth, float min_weight, const ksg_render_out* d_out, void* cuda_stream) {
+  RenderCam c{};
+  { const int rca = render_args(h, T_G_C_host, K_host, width, height, min_depth, max_depth, min_weight, d_out, &c); if (rca) return rca; }
+  const bool at_hit = query_wanted(d_out->at_hit);
+  if (at_hit && !d_out->points_G) return h->fail(KSG_ERR_INVALID_ARGUMENT, "render: an at_hit output needs points_G (the query reads it)");
+  if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
+  if (!d_out->depth && !d_out->points_G) return KSG_OK;
+  KSG_CUDA(cudaSetDevice(h->device));
+  launch_render(h, c, d_out->depth, d_out->points_G, d_out->at_hit, cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream);
   KSG_CUDA(cudaGetLastError());
   return KSG_OK;
 }
