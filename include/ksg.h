@@ -379,6 +379,25 @@ int32_t ksg_render_view(ksg_integrator* h, const float* T_G_C, const double* K, 
 int32_t ksg_render_view_device(ksg_integrator* h, const float* T_G_C_host, const double* K_host, int32_t width, int32_t height,
                                float min_depth, float max_depth, float min_weight, const ksg_render_out* d_out, void* cuda_stream);
 
+/* Batch Euclidean signed distance field of the device map (what a planner reads: the signed distance to the nearest surface at every
+ * observed voxel).  A closed-form minimum, not voxblox's queue propagation: unpinned; csrc/ksg_esdf.cuh states the rules and the error
+ * bound.  vs = voxel_size, m = max_distance, W = ceil(m / vs) + 1 (in double):
+ *   - observed voxel: weight > min_weight in an allocated block; surface voxel (site): observed, with an observed face neighbour on the
+ *     other side of zero (0 counts as non-positive) whose |distance| is not smaller;
+ *   - Q = the least integer squared voxel offset to a site;
+ *   - for the nb * V voxels of the allocated blocks, in ksg_export_blocks order (block_index as it fills it) and linear voxel order:
+ *     unobserved: distance NaN, flags 0; site: the TSDF distance, OBSERVED | SURFACE; otherwise mag = fl(sqrtf((float)Q) * vs) when a
+ *     site lies in the window max(|dx|, |dy|, |dz|) <= W and mag < m, else mag = m with CAPPED; distance = +mag if the TSDF distance
+ *     is > 0, else -mag.  Exact and independent of the order of computation.
+ * Any output may be NULL and an unwanted array is never written.  The call completes the pending frame, reads the map and never writes
+ * it, and returns when done.  Rejected (KSG_ERR_INVALID_ARGUMENT): a NULL handle, a NaN or negative min_weight, a non-finite or
+ * non-positive max_distance, W > 512 (bounds the work per voxel, 3 (2W + 1) candidates, and the block dilation), capacity_blocks < nb
+ * (as ksg_export_blocks), a spatially sharded integrator (as ksg_query_points).  An empty map, or neither distance nor flags wanted,
+ * launches nothing; otherwise the call makes 4 kernel launches. */
+enum { KSG_ESDF_OBSERVED = 1, KSG_ESDF_SURFACE = 2, KSG_ESDF_CAPPED = 4 };
+int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance, int64_t capacity_blocks, int32_t* block_index,
+                         float* distance, uint8_t* flags);
+
 /* Remove every block but keep the integrator: what Layer::removeAllBlocks() on both layers does to a live reference integrator.  The
  * fast integrator's two per-scan approximate sets (members of the integrator, fast.h:114-130) keep their contents and offsets, so the
  * next frame is integrated exactly as the reference integrator object would integrate it into its emptied layers.  Used by the

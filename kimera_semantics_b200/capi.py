@@ -94,6 +94,9 @@ KSG_QUERY_ALLOCATED = 1
 KSG_QUERY_OBSERVED = 2
 KSG_QUERY_INTERPOLATED = 4
 KSG_QUERY_GRADIENT = 8
+KSG_ESDF_OBSERVED = 1
+KSG_ESDF_SURFACE = 2
+KSG_ESDF_CAPPED = 4
 QUERY_FIELDS = ("flags", "tsdf_distance", "tsdf_weight", "tsdf_rgba", "sem_label", "sem_priors", "sem_rgba", "distance", "gradient")
 
 
@@ -290,6 +293,8 @@ def load_library(path: Optional[str] = None):
     lib.ksg_render_view_device.argtypes = [H, fp, dp, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float, C.POINTER(KsgRenderOut),
                                            C.c_void_p]
     lib.ksg_render_view_device.restype = C.c_int32
+    lib.ksg_compute_esdf.argtypes = [H, C.c_float, C.c_float, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.ksg_compute_esdf.restype = C.c_int32
     lib.ksg_clear_map.argtypes = [H]
     lib.ksg_clear_map.restype = C.c_int32
     lib.ksg_build_info.argtypes = []
@@ -306,7 +311,7 @@ KSG_SYMBOLS = ["ksg_default_config", "ksg_create", "ksg_destroy", "ksg_last_erro
                "ksg_unordered_map_schedule", "ksg_integrate_depth_k64", "ksg_integrate_depth_device_k64",
                "ksg_debug_chain_sum", "ksg_debug_tsdf_batch", "ksg_debug_apply_routes", "ksg_debug_fast_timeline", "ksg_integrate_depth_async", "ksg_wait_frame",
                "ksg_device_map_view", "ksg_merge_blocks_device", "ksg_copy_map_device", "ksg_integrate_image", "ksg_set_update_log", "ksg_fetch_update_log", "ksg_evaluate_labels", "ksg_extract_mesh", "ksg_clear_map", "ksg_copy_update_log_device", "ksg_merge_voxels_device",
-               "ksg_query_points", "ksg_query_points_device", "ksg_render_view", "ksg_render_view_device"]
+               "ksg_query_points", "ksg_query_points_device", "ksg_render_view", "ksg_render_view_device", "ksg_compute_esdf"]
 
 
 def debug_chain_sum(terms: np.ndarray, s0: float, lib=None) -> np.float32:
@@ -650,6 +655,16 @@ class Integrator:
                                               lab.ctypes.data_as(C.c_void_p), b, bidx.ctypes.data_as(C.c_void_p), first.ctypes.data_as(C.c_void_p),
                                               C.byref(nv), C.byref(nb)), "ksg_extract_mesh")
         return {"vertices": vtx, "rgba": rgba, "labels": lab, "block_index": bidx, "block_first": first}
+
+    def esdf(self, max_distance: float, min_weight: float = 1e-4) -> Dict[str, np.ndarray]:
+        """Batch Euclidean signed distance field of the map (ksg_compute_esdf): dict(block_index [nb, 3] i32 in export order,
+        distance [nb, V] f32 (NaN where unobserved), flags [nb, V] u8 (KSG_ESDF_*))."""
+        nb = self.num_blocks()
+        V = self.cfg.voxels_per_side ** 3
+        out = {"block_index": np.zeros((nb, 3), np.int32), "distance": np.zeros((nb, V), np.float32), "flags": np.zeros((nb, V), np.uint8)}
+        self._check(self.lib.ksg_compute_esdf(self.handle, min_weight, max_distance, nb, *(C.c_void_p(a.ctypes.data) for a in out.values())),
+                    "ksg_compute_esdf")
+        return out
 
     def query_points(self, xyz, min_weight: float = 1e-4, priors: bool = True) -> Dict[str, np.ndarray]:
         """Point queries on the device map (ksg_query_points): dict(flags [n] u8 (KSG_QUERY_*), tsdf_distance / tsdf_weight [n] f32,

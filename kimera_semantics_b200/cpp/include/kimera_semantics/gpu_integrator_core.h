@@ -58,6 +58,11 @@ class GpuIntegratorCore {
   };
   bool renderView(const vxb::Transformation& T_G_C, const double K[4], int w, int h, float min_depth, float max_depth, float min_weight,
                   RenderResult* result);
+  // Batch Euclidean signed distance field of the device map (ksg_compute_esdf, csrc/ksg_esdf.cuh), read-only like queryPoints: works in
+  // kLazy mode without syncLayers().  Replaces the contents of *esdf_layer (same voxel size and voxels_per_side as the map) with one
+  // block per allocated map block: observed = OBSERVED, fixed = SURFACE, distance as computed; an unobserved voxel is voxblox's default
+  // EsdfVoxel (distance 0, not observed).
+  bool computeEsdf(float min_weight, float max_distance, vxb::Layer<vxb::EsdfVoxel>* esdf_layer);
   int64_t lastVoxelUpdates() const { return last_voxel_updates_; }
   ksg_integrator* handle() { return handle_; }
 

@@ -21,7 +21,8 @@ namespace map_io {
 static const char kMagic[4] = {'K', 'S', 'G', 'M'};
 static const uint32_t kVersion = 1u;
 
-inline std::vector<vxb::BlockIndex> sortedBlocks(const vxb::Layer<vxb::TsdfVoxel>& layer) {
+template <typename VoxelType>
+inline std::vector<vxb::BlockIndex> sortedBlocks(const vxb::Layer<VoxelType>& layer) {
   vxb::BlockIndexList all;
   layer.getAllAllocatedBlocks(&all);
   std::vector<vxb::BlockIndex> v(all.begin(), all.end());

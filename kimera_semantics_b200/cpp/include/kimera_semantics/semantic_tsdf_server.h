@@ -114,6 +114,13 @@ class SemanticTsdfServer {
     return gpu().renderView(T_G_C, K, w, h, min_depth, max_depth, min_weight, result);
   }
 
+  // voxblox's EsdfServer::updateEsdfBatch(full_euclidean_distance = true), the last step of the reference's offline driver
+  // (kimera_semantics_rosbag.cpp:160-166): the ESDF of the whole map, computed on the device from the device map
+  // (GpuIntegratorCore::computeEsdf, csrc/ksg_esdf.cuh; not voxblox's queue algorithm): needs no updateLayers().
+  bool updateEsdfBatch(vxb::Layer<vxb::EsdfVoxel>* esdf_layer, float max_distance, float min_weight = 1e-4f) {
+    return gpu().computeEsdf(min_weight, max_distance, esdf_layer);
+  }
+
   vxb::Layer<vxb::TsdfVoxel>* getTsdfLayerPtr() { return tsdf_layer_.get(); }
   vxb::Layer<SemanticVoxel>* getSemanticLayerPtr() { return semantic_layer_.get(); }
   vxb::TsdfIntegratorBase* getIntegratorPtr() { return tsdf_integrator_.get(); }

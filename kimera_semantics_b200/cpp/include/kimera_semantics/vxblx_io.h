@@ -6,7 +6,8 @@
 //   file      = varint32 N, then N length-delimited messages (varint32 size + bytes): one LayerProto, then N - 1 BlockProto
 //   LayerProto: 1 double voxel_size, 2 uint32 voxels_per_side, 3 string type ("tsdf")
 //   BlockProto: 1 int32 voxels_per_side, 2 double voxel_size, 3/4/5 double origin_x/y/z, 6 bool has_data, 7 repeated uint32 voxel_data
-//               (packed); a TSDF voxel is 3 words: distance bits, weight bits, (r << 24 | g << 16 | b << 8 | a)
+//               (packed); a TSDF voxel is 3 words: distance bits, weight bits, (r << 24 | g << 16 | b << 8 | a); an ESDF voxel
+//               (saveEsdfLayer, LayerProto type "esdf") is 2 words: distance bits, observed | hallucinated << 8 | in_queue << 16 | fixed << 24
 // tests/test_shim_cpu.py parses a file written here with google.protobuf against exactly this schema.  Host-only code.
 #pragma once
 #include <cmath>
@@ -75,8 +76,9 @@ struct Reader {
 };
 }  // namespace wire
 
-// voxblox::io::SaveLayer for Layer<TsdfVoxel>: all allocated blocks, (z, y, x) order (voxblox: hash-map order; readers do not depend on it)
-inline bool saveTsdfLayer(const std::string& path, const vxb::Layer<vxb::TsdfVoxel>& layer) {
+// The file head and the blocks of voxblox::io::SaveLayer; `words(block, &data)` appends a block's packed voxel_data.
+template <typename VoxelType, typename Words>
+bool saveLayer(const std::string& path, const vxb::Layer<VoxelType>& layer, const char* type, Words words) {
   std::ofstream o(path.c_str(), std::ios::binary | std::ios::trunc);
   if (!o.good()) return false;
   const std::vector<vxb::BlockIndex> blocks = map_io::sortedBlocks(layer);
@@ -84,13 +86,13 @@ inline bool saveTsdfLayer(const std::string& path, const vxb::Layer<vxb::TsdfVox
   wire::varint(&head, 1u + blocks.size());
   wire::f64(&msg, 1, (double)layer.voxel_size());
   wire::u64(&msg, 2, (uint64_t)layer.voxels_per_side());
-  wire::bytes(&msg, 3, "tsdf");
+  wire::bytes(&msg, 3, type);
   wire::varint(&head, msg.size());
   o.write(head.data(), (std::streamsize)head.size());
   o.write(msg.data(), (std::streamsize)msg.size());
   std::string data;
   for (const vxb::BlockIndex& bi : blocks) {
-    const vxb::Block<vxb::TsdfVoxel>::ConstPtr b = layer.getBlockPtrByIndex(bi);
+    const typename vxb::Block<VoxelType>::ConstPtr b = layer.getBlockPtrByIndex(bi);
     msg.clear();
     wire::u64(&msg, 1, (uint64_t)b->voxels_per_side());
     wire::f64(&msg, 2, (double)b->voxel_size());
@@ -99,15 +101,7 @@ inline bool saveTsdfLayer(const std::string& path, const vxb::Layer<vxb::TsdfVox
     wire::f64(&msg, 5, (double)b->origin().z());
     wire::u64(&msg, 6, b->has_data() ? 1u : 0u);
     data.clear();
-    for (size_t v = 0; v < b->num_voxels(); ++v) {
-      const vxb::TsdfVoxel& t = b->getVoxelByLinearIndex(v);
-      uint32_t d, w;
-      std::memcpy(&d, &t.distance, 4);
-      std::memcpy(&w, &t.weight, 4);
-      wire::varint(&data, d);
-      wire::varint(&data, w);
-      wire::varint(&data, ((uint32_t)t.color.r << 24) | ((uint32_t)t.color.g << 16) | ((uint32_t)t.color.b << 8) | (uint32_t)t.color.a);
-    }
+    words(*b, &data);
     wire::bytes(&msg, 7, data);
     head.clear();
     wire::varint(&head, msg.size());
@@ -115,6 +109,36 @@ inline bool saveTsdfLayer(const std::string& path, const vxb::Layer<vxb::TsdfVox
     o.write(msg.data(), (std::streamsize)msg.size());
   }
   return o.good();
+}
+
+// voxblox::io::SaveLayer for Layer<EsdfVoxel> (what EsdfServer::saveMap writes beside the TSDF): restated from knowledge of voxblox's
+// Block<EsdfVoxel> serialisation, unpinned like saveTsdfLayer.  Two words per voxel: the distance bits, then
+// observed | hallucinated << 8 | in_queue << 16 | fixed << 24.
+inline bool saveEsdfLayer(const std::string& path, const vxb::Layer<vxb::EsdfVoxel>& layer) {
+  return saveLayer(path, layer, "esdf", [](const vxb::Block<vxb::EsdfVoxel>& b, std::string* data) {
+    for (size_t v = 0; v < b.num_voxels(); ++v) {
+      const vxb::EsdfVoxel& e = b.getVoxelByLinearIndex(v);
+      uint32_t d;
+      std::memcpy(&d, &e.distance, 4);
+      wire::varint(data, d);
+      wire::varint(data, (uint32_t)e.observed | ((uint32_t)e.hallucinated << 8) | ((uint32_t)e.in_queue << 16) | ((uint32_t)e.fixed << 24));
+    }
+  });
+}
+
+// voxblox::io::SaveLayer for Layer<TsdfVoxel>: all allocated blocks, (z, y, x) order (voxblox: hash-map order; readers do not depend on it)
+inline bool saveTsdfLayer(const std::string& path, const vxb::Layer<vxb::TsdfVoxel>& layer) {
+  return saveLayer(path, layer, "tsdf", [](const vxb::Block<vxb::TsdfVoxel>& b, std::string* data) {
+    for (size_t v = 0; v < b.num_voxels(); ++v) {
+      const vxb::TsdfVoxel& t = b.getVoxelByLinearIndex(v);
+      uint32_t d, w;
+      std::memcpy(&d, &t.distance, 4);
+      std::memcpy(&w, &t.weight, 4);
+      wire::varint(data, d);
+      wire::varint(data, w);
+      wire::varint(data, ((uint32_t)t.color.r << 24) | ((uint32_t)t.color.g << 16) | ((uint32_t)t.color.b << 8) | (uint32_t)t.color.a);
+    }
+  });
 }
 
 // voxblox::io::LoadLayer / LoadBlocksFromFile (kReplace) for Layer<TsdfVoxel>: the layer must have the file's voxel size and voxels per

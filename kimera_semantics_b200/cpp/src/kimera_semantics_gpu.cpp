@@ -348,6 +348,30 @@ bool GpuIntegratorCore::renderView(const vxb::Transformation& T_G_C, const doubl
   return ksg_render_view(handle_, T, K, w, h, min_depth, max_depth, min_weight, &out) == KSG_OK;
 }
 
+bool GpuIntegratorCore::computeEsdf(float min_weight, float max_distance, vxb::Layer<vxb::EsdfVoxel>* esdf) {
+  if (!esdf || esdf->voxels_per_side() != tsdf_layer_->voxels_per_side()) return false;
+  const int64_t nb = ksg_num_blocks(handle_);
+  const size_t V = esdf->voxels_per_side() * esdf->voxels_per_side() * esdf->voxels_per_side();
+  std::vector<int32_t> index(3 * (size_t)nb);
+  std::vector<float> distance((size_t)nb * V);
+  std::vector<uint8_t> flags((size_t)nb * V);
+  if (ksg_compute_esdf(handle_, min_weight, max_distance, nb, index.data(), distance.data(), flags.data()) != KSG_OK) return false;
+  esdf->removeAllBlocks();
+  for (int64_t b = 0; b < nb; ++b) {
+    vxb::Block<vxb::EsdfVoxel>::Ptr blk = esdf->allocateNewBlock(vxb::BlockIndex(index[3 * b], index[3 * b + 1], index[3 * b + 2]));
+    blk->has_data() = true;
+    for (size_t v = 0; v < V; ++v) {
+      const uint8_t f = flags[b * V + v];
+      if (!(f & KSG_ESDF_OBSERVED)) continue;
+      vxb::EsdfVoxel& e = blk->getVoxelByLinearIndex(v);
+      e.distance = distance[b * V + v];
+      e.observed = true;
+      e.fixed = (f & KSG_ESDF_SURFACE) != 0;
+    }
+  }
+  return true;
+}
+
 void GpuIntegratorCore::uploadLayers() {
   vxb::BlockIndexList blocks;
   tsdf_layer_->getAllAllocatedBlocks(&blocks);

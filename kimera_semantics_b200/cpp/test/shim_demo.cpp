@@ -1,6 +1,7 @@
 // Drives the drop-in C++ API exactly the way SemanticTsdfServer does (kimera_semantics_ros/src/semantic_tsdf_server.cpp:58-79):
 // build both layers, SemanticTsdfIntegratorFactory::create(method, ...), then integratePointCloud per frame.
 //   shim_demo <fast|merged|bogus> <frames.bin> <out.bin> [lazy] [--load ckpt] [--save ckpt] [--skip N] [--query in out] [--render in out]
+//             [--esdf max_distance out]
 //     --load: SemanticTsdfServer::loadMap before the first frame; --save: saveMap after the last; --skip: ignore the first N frames
 //     --depth file: instead of the clouds of frames.bin (whose frame count must then be 0) feed depth + label frames:
 //              int32 n, int32 width, int32 height, double K[4], then per frame float T[7], float depth[w*h], uint8 label[w*h]
@@ -11,6 +12,8 @@
 //     --render in out: after the last frame (also before any layer sync) SemanticTsdfServer::renderView with `in` = float T_G_C[7],
 //              double K[4], int32 w, int32 h, float min_depth, max_depth, min_weight; `out` = depth[n] f32, points_G[3n] f32, then the
 //              arrays of --query's output for the n = w * h hit points
+//     --esdf max_distance out: after the last frame (also before any layer sync) SemanticTsdfServer::updateEsdfBatch (min_weight 1e-4),
+//              then vxblx_io::saveEsdfLayer to `out` - the reference driver's last step (kimera_semantics_rosbag.cpp:160-166)
 // frames.bin : int32 n_frames, float voxel_size, int32 vps, int32 n_palette, palette n*(r,g,b,a,id), int32 n_dynamic, ids...,
 //              then per frame: int32 n, float T[7], float xyz[3n], uint8 rgba[4n]
 // out.bin    : int32 n_blocks, then per block (sorted z,y,x): int32 idx[3], per voxel: float d, float w, u8 rgba[4], u8 label,
@@ -26,6 +29,7 @@
 #include "kimera_semantics/semantic_tsdf_integrator_fast.h"
 #include "kimera_semantics/semantic_tsdf_integrator_merged.h"
 #include "kimera_semantics/semantic_tsdf_server.h"
+#include "kimera_semantics/vxblx_io.h"
 
 using namespace kimera;
 template <typename T> static T rd(std::ifstream& f) { T v; f.read(reinterpret_cast<char*>(&v), sizeof(T)); return v; }
@@ -48,7 +52,8 @@ int main(int argc, char** argv) {
   config.default_truncation_distance = 4.0f * voxel_size;  // voxblox_ros
   bool lazy = false;
   const char *load_path = nullptr, *save_path = nullptr, *depth_path = nullptr, *query_in = nullptr, *query_out = nullptr;
-  const char *render_in = nullptr, *render_out = nullptr;
+  const char *render_in = nullptr, *render_out = nullptr, *esdf_out = nullptr;
+  float esdf_max_distance = 0.0f;
   int skip = 0;
   for (int a = 4; a < argc; ++a) {
     if (std::strcmp(argv[a], "lazy") == 0) lazy = true;
@@ -58,6 +63,7 @@ int main(int argc, char** argv) {
     else if (std::strcmp(argv[a], "--depth") == 0 && a + 1 < argc) depth_path = argv[++a];
     else if (std::strcmp(argv[a], "--query") == 0 && a + 2 < argc) { query_in = argv[++a]; query_out = argv[++a]; }
     else if (std::strcmp(argv[a], "--render") == 0 && a + 2 < argc) { render_in = argv[++a]; render_out = argv[++a]; }
+    else if (std::strcmp(argv[a], "--esdf") == 0 && a + 2 < argc) { esdf_max_distance = (float)std::atof(argv[++a]); esdf_out = argv[++a]; }
   }
   SemanticTsdfServer::Params params;
   params.tsdf_voxel_size = voxel_size;
@@ -151,6 +157,12 @@ int main(int argc, char** argv) {
     size_t hits = 0;
     for (float d : rr.depth) hits += (d == d) ? 1 : 0;
     std::printf("render: %dx%d pixels, %zu hits%s\n", w, h, hits, lazy ? " (host layers not synchronised)" : "");
+  }
+  if (esdf_out) {
+    vxb::Layer<vxb::EsdfVoxel> esdf(tsdf_layer.voxel_size(), tsdf_layer.voxels_per_side());
+    KSG_CHECK(server.updateEsdfBatch(&esdf, esdf_max_distance)) << "esdf failed";
+    KSG_CHECK(vxblx_io::saveEsdfLayer(esdf_out, esdf)) << "cannot save " << esdf_out;
+    std::printf("esdf: %zu blocks%s\n", esdf.getNumberOfAllocatedBlocks(), lazy ? " (host layers not synchronised)" : "");
   }
   if (lazy) server.updateLayers();
   {

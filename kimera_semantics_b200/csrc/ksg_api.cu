@@ -31,6 +31,7 @@
 #include "ksg_mesh.cuh"
 #include "ksg_query.cuh"
 #include "ksg_render.cuh"
+#include "ksg_esdf.cuh"
 
 using namespace ksg;
 
@@ -1972,6 +1973,140 @@ int32_t ksg_render_view_device(ksg_integrator* h, const float* T_G_C_host, const
   KSG_CUDA(cudaSetDevice(h->device));
   launch_render(h, c, d_out->depth, d_out->points_G, d_out->at_hit, cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream);
   KSG_CUDA(cudaGetLastError());
+  return KSG_OK;
+}
+
+namespace {
+// The work sets of the x and y passes and the neighbour tables of the three passes (ksg_esdf.cuh), from the keys of the allocated blocks
+// (output order) and which of them hold a site.  Blocks outside the key range hold no site, and neither does any block sharing their
+// out-of-range coordinate, so their pass results are "none" and they are left out.
+struct EsdfWork {
+  int64_t n_x = 0, n_y = 0;
+  std::vector<int> tx, ty, tz;   // per block of the x / y / z pass: 2 Rb + 1 indices into the previous stage, -1 = none
+
+  void build(const std::vector<I3>& alloc, const std::vector<uint8_t>& has_site, int Rb) {
+    const int span = 2 * Rb + 1;
+    auto moved = [](I3 b, int axis, int k) { if (axis == 0) b.x += k; else if (axis == 1) b.y += k; else b.z += k; return b; };
+    std::unordered_map<uint64_t, int> site_at;      // site block -> its index in alloc
+    std::unordered_map<uint64_t, char> near_x;      // within Rb along x of a site block
+    for (size_t a = 0; a < alloc.size(); ++a) {
+      if (!has_site[a]) continue;
+      site_at[pack_key(alloc[a])] = (int)a;
+      for (int k = -Rb; k <= Rb; ++k) {
+        const I3 b = moved(alloc[a], 0, k);
+        if (key_in_range(b)) near_x[pack_key(b)] = 1;
+      }
+    }
+    // Y: within Rb along z of an allocated block, with a near_x block within Rb along y
+    std::unordered_map<uint64_t, int> y_at;         // -1: looked at and left out
+    std::vector<I3> ys;
+    for (const I3& a : alloc)
+      for (int k = -Rb; k <= Rb; ++k) {
+        const I3 b = moved(a, 2, k);
+        if (!key_in_range(b) || y_at.count(pack_key(b))) continue;
+        bool keep = false;
+        for (int j = -Rb; j <= Rb && !keep; ++j) {
+          const I3 c = moved(b, 1, j);
+          keep = key_in_range(c) && near_x.count(pack_key(c));
+        }
+        y_at[pack_key(b)] = keep ? (int)ys.size() : -1;
+        if (keep) ys.push_back(b);
+      }
+    // X: within Rb along y of a Y block, and near_x
+    std::unordered_map<uint64_t, int> x_at;
+    std::vector<I3> xs;
+    for (const I3& y : ys)
+      for (int j = -Rb; j <= Rb; ++j) {
+        const I3 b = moved(y, 1, j);
+        if (!key_in_range(b) || !near_x.count(pack_key(b)) || x_at.count(pack_key(b))) continue;
+        x_at[pack_key(b)] = (int)xs.size();
+        xs.push_back(b);
+      }
+    n_x = (int64_t)xs.size();
+    n_y = (int64_t)ys.size();
+    auto table = [&](const std::vector<I3>& blocks, int axis, const std::unordered_map<uint64_t, int>& prev, std::vector<int>* t) {
+      t->assign(blocks.size() * span, -1);
+      for (size_t i = 0; i < blocks.size(); ++i)
+        for (int k = -Rb; k <= Rb; ++k) {
+          const I3 b = moved(blocks[i], axis, k);
+          if (!key_in_range(b)) continue;
+          const auto it = prev.find(pack_key(b));
+          if (it != prev.end()) (*t)[i * span + Rb + k] = it->second;
+        }
+    };
+    table(xs, 0, site_at, &tx);
+    table(ys, 1, x_at, &ty);
+    table(alloc, 2, y_at, &tz);
+  }
+};
+
+int esdf_grid(ksg_integrator* h, int64_t blocks) {
+  const int64_t items = blocks * (int64_t)h->dc.vps * h->dc.vps * h->dc.vps;
+  return (int)std::max<int64_t>(1, std::min<int64_t>((items + kEsdfThreads - 1) / kEsdfThreads, (int64_t)h->sm_count * 16));
+}
+}  // namespace
+
+int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance, int64_t capacity_blocks, int32_t* block_index,
+                         float* distance, uint8_t* flags) {
+  if (!h) return KSG_ERR_INVALID_ARGUMENT;
+  if (!(min_weight >= 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: NaN or negative min_weight");
+  if (!std::isfinite(max_distance) || !(max_distance > 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: max_distance must be finite and > 0");
+  const double Wd = std::ceil((double)max_distance / (double)h->dc.voxel_size) + 1.0;
+  if (!(Wd <= (double)kEsdfMaxWindow)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: ceil(max_distance / voxel_size) + 1 > 512");
+  if (h->dc.shard_count > 1) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: a sharded integrator holds only its own tiles");
+  KSG_CUDA(cudaSetDevice(h->device));
+  KSG_CUDA(cudaDeviceSynchronize());
+  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  const int64_t nb = h->num_blocks;
+  if (nb > capacity_blocks) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: block capacity too small");
+  if (nb == 0) return KSG_OK;
+  std::vector<int> order;
+  std::vector<int32_t> index((size_t)(3 * nb));
+  { const int rco = slots_zyx(h, &order, index.data()); if (rco) return rco; }
+  if (block_index) std::memcpy(block_index, index.data(), sizeof(int32_t) * 3 * nb);
+  if (!distance && !flags) return KSG_OK;
+  const int W = (int)Wd, vps = h->dc.vps, Rb = (W + vps - 1) / vps;
+  const size_t V = (size_t)vps * vps * vps;
+  Resources tmp;
+  int* d_slots = nullptr; uint8_t* d_site = nullptr; uint8_t* d_has = nullptr;
+  KSG_CUDA(tmp.device(&d_slots, nb));
+  KSG_CUDA(tmp.device(&d_site, nb * V));
+  KSG_CUDA(tmp.device(&d_has, nb));
+  cudaStream_t s = h->own_stream;
+  KSG_CUDA(cudaMemcpyAsync(d_slots, order.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s));
+  ++h->n_launches;
+  k_esdf_sites<<<(int)std::min<int64_t>(nb, (int64_t)h->sm_count * 8), kEsdfThreads, 0, s>>>(h->dc, h->map, d_slots, (int)nb, min_weight,
+                                                                                              d_site, d_has);
+  std::vector<uint8_t> has((size_t)nb);
+  KSG_CUDA(cudaMemcpyAsync(has.data(), d_has, nb, cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
+  KSG_CUDA(cudaGetLastError());
+  std::vector<I3> alloc((size_t)nb);
+  for (int64_t i = 0; i < nb; ++i) alloc[i] = I3{index[3 * i], index[3 * i + 1], index[3 * i + 2]};
+  EsdfWork wk;
+  wk.build(alloc, has, Rb);
+  int *d_tx = nullptr, *d_ty = nullptr, *d_tz = nullptr, *d_a = nullptr, *d_b = nullptr;
+  float* d_dist = nullptr; uint8_t* d_flags = nullptr;
+  KSG_CUDA(tmp.device(&d_tx, wk.tx.size()));
+  KSG_CUDA(tmp.device(&d_ty, wk.ty.size()));
+  KSG_CUDA(tmp.device(&d_tz, wk.tz.size()));
+  KSG_CUDA(tmp.device(&d_a, wk.n_x * V));
+  KSG_CUDA(tmp.device(&d_b, wk.n_y * V));
+  if (distance) KSG_CUDA(tmp.device(&d_dist, nb * V));
+  if (flags) KSG_CUDA(tmp.device(&d_flags, nb * V));
+  KSG_CUDA(cudaMemcpyAsync(d_tx, wk.tx.data(), sizeof(int) * wk.tx.size(), cudaMemcpyHostToDevice, s));
+  KSG_CUDA(cudaMemcpyAsync(d_ty, wk.ty.data(), sizeof(int) * wk.ty.size(), cudaMemcpyHostToDevice, s));
+  KSG_CUDA(cudaMemcpyAsync(d_tz, wk.tz.data(), sizeof(int) * wk.tz.size(), cudaMemcpyHostToDevice, s));
+  const EsdfOut none{nullptr, nullptr, nullptr, 0.0f, 0.0f};
+  const EsdfOut eo{d_dist, d_flags, d_slots, min_weight, max_distance};
+  h->n_launches += 3;
+  k_esdf_pass<0><<<esdf_grid(h, wk.n_x), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_x, W, Rb, d_tx, d_site, nullptr, d_a, nullptr, none);
+  k_esdf_pass<1><<<esdf_grid(h, wk.n_y), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_y, W, Rb, d_ty, nullptr, d_a, d_b, nullptr, none);
+  k_esdf_pass<2><<<esdf_grid(h, nb), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)nb, W, Rb, d_tz, nullptr, d_b, nullptr, d_site, eo);
+  KSG_CUDA(cudaGetLastError());
+  if (distance) KSG_CUDA(cudaMemcpyAsync(distance, d_dist, sizeof(float) * nb * V, cudaMemcpyDeviceToHost, s));
+  if (flags) KSG_CUDA(cudaMemcpyAsync(flags, d_flags, nb * V, cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
 }
 
