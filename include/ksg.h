@@ -265,7 +265,8 @@ int32_t ksg_copy_map_device(ksg_integrator* h, void* d_dst_pool, void* d_dst_key
 /* Update log: the cheap way to keep HOST layers in step with the device map after every call (the reference's contract, base.cpp:257-265:
  * on return the caller reads the host Layer<> objects).  With a log of `capacity_voxels` entries switched on, every integrate call leaves
  * one entry per voxel it updated (final distance, weight, colours, label and log-probabilities): a fraction of the bytes of the updated
- * blocks.  Both integrators keep it: `fast` in its apply kernel (entries grouped by tile), `merged` in one extra pass behind its apply
+ * blocks.  Both integrators keep it: `fast` in its apply kernel (no order across tiles: a tile's entries come in ascending voxel order,
+ * in one contiguous run per 512 of its update records, and other tiles' runs may fall between them), `merged` in one extra pass behind its apply
  * kernels (entries in (block index, tile, voxel) order, the same bytes on every run and whichever apply route ran; with spatial
  * sharding, only the tiles this rank owns).  ksg_fetch_update_log completes the last frame, copies its entries to page-locked host memory owned by the library (two DMA
  * transfers) and returns pointers that stay valid until the next call on this handle; *n = -1 and KSG_ERR_SCRATCH_FULL when the frame

@@ -223,7 +223,7 @@ void GpuIntegratorCore::syncAfterCall() {
   for (int64_t i = 0; i < n; ++i) {
     const ksg_voxel_update& u = up[i];
     const vxb::BlockIndex bi(u.block_index[0], u.block_index[1], u.block_index[2]);
-    if (!(bi == last_bi)) {           // entries come tile by tile (`merged`: block by block): the block changes rarely
+    if (!(bi == last_bi)) {           // entries come in runs of one tile (`merged`: block by block): the block changes rarely; any order is correct
       last_bi = bi;
       tb = tsdf_layer_->allocateBlockPtrByIndex(bi);        // base.cpp:257-265: new blocks appear in both layers
       sb = semantic_layer_->allocateBlockPtrByIndex(bi);
