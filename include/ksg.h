@@ -399,6 +399,57 @@ enum { KSG_ESDF_OBSERVED = 1, KSG_ESDF_SURFACE = 2, KSG_ESDF_CAPPED = 4 };
 int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance, int64_t capacity_blocks, int32_t* block_index,
                          float* distance, uint8_t* flags);
 
+/* The ESDF kept on the device and brought up to date from the blocks that changed (what voxblox's EsdfServer::updateEsdf does while the
+ * map grows).  The layer holds, per pool slot, the distance, the flags and the site byte of every voxel; the first ksg_update_esdf
+ * allocates it (max_blocks rows) and ksg_destroy frees it.  After every update the layer equals what ksg_compute_esdf(min_weight,
+ * max_distance) returns for the map at that moment, bit for bit: same definition, same kernels (csrc/ksg_esdf.cuh states the incremental
+ * rule and why it is exact).
+ * ksg_update_esdf: rejects what ksg_compute_esdf rejects (a NULL handle, a NaN or negative min_weight, a non-finite or non-positive
+ * max_distance, W > 512, a sharded integrator), completes the pending frame, updates the layer and returns when done.  The update is
+ * full (every block recomputed) on the first call, after a change of (min_weight, max_distance), and after any ksg_clear_map, ksg_reset
+ * or ksg_import_blocks since the last update.  Otherwise it recomputes the site bytes of the blocks touched or allocated since the last
+ * update and of their face neighbours, and the output of the blocks that can have changed; nothing changed: no launch.  Otherwise 4
+ * kernel launches.  `stats` (may be NULL) receives the counts below.  A call that fails after its argument checks (a device error, an
+ * allocation that fails) leaves the layer untrusted: export and query are refused and the next update is full.
+ * ksg_export_esdf: the layer as of the last update.  changed_only = 0: every block it covers, in ksg_export_blocks order (z, y, x);
+ * changed_only = 1: only the blocks whose output the last update rewrote (z_blocks), in (z, y, x) order.  *n_blocks (may be NULL) gets the
+ * block count; with all three arrays NULL the call only sizes.  Rejected: capacity_blocks smaller than the count when an array is wanted,
+ * and a call before any update (or after a clear / reset or a failed update with no successful update since).  One kernel launch when
+ * distance or flags is wanted. */
+typedef struct ksg_esdf_stats {
+  int64_t blocks;            /* allocated blocks the layer now covers (= ksg_num_blocks) */
+  int64_t full;              /* 1: recomputed from scratch (first call, new parameters, after clear / reset / import) */
+  int64_t changed_blocks;    /* blocks touched, or allocated, since the previous update */
+  int64_t site_blocks;       /* blocks whose site bytes were recomputed */
+  int64_t site_changed;      /* ... of which at least one site byte changed */
+  int64_t x_blocks, y_blocks, z_blocks;   /* work sets of the three passes; z_blocks = blocks whose output was rewritten */
+  int64_t reserved[4];
+} ksg_esdf_stats;
+int32_t ksg_update_esdf(ksg_integrator* h, float min_weight, float max_distance, ksg_esdf_stats* stats);
+int32_t ksg_export_esdf(ksg_integrator* h, int32_t changed_only, int64_t capacity_blocks, int64_t* n_blocks, int32_t* block_index,
+                        float* distance, uint8_t* flags);
+
+/* Point queries on the device ESDF layer: the rules of ksg_query_points (containing voxel floor(p / vs + 1e-6), the same trilinear form
+ * and corner order, the same +-vs central differences, NaN and 0 for what is not valid, unwanted arrays never written) with the ESDF
+ * distance in place of the TSDF distance:
+ *   - flags: KSG_QUERY_ALLOCATED when the containing block is in the layer (a block allocated after the last update is not: the query
+ *     reads the layer as of that update and does not bring it up to date), KSG_QUERY_OBSERVED when the voxel is KSG_ESDF_OBSERVED there
+ *     (CAPPED voxels are observed and hold +-max_distance, as in voxblox), KSG_QUERY_INTERPOLATED / KSG_QUERY_GRADIENT as for the TSDF
+ *     with "observed" in that sense;
+ *   - voxel_flags / voxel_distance: KSG_ESDF_* and the ESDF distance of the containing voxel (0 / NaN outside the layer).
+ * Rejected (KSG_ERR_INVALID_ARGUMENT): a NULL handle or out, n < 0, n > 0 with NULL points, a sharded integrator, and a call before any
+ * update (or after a clear / reset or a failed update with no successful update since).  Stream order, the NULL stream and the host / device split are those of
+ * ksg_query_points / ksg_query_points_device; one kernel launch when anything is wanted. */
+typedef struct ksg_esdf_query_out {
+  uint8_t* flags;          /* n: KSG_QUERY_ALLOCATED | KSG_QUERY_OBSERVED | KSG_QUERY_INTERPOLATED | KSG_QUERY_GRADIENT */
+  uint8_t* voxel_flags;    /* n: KSG_ESDF_* of the containing voxel, 0 when its block is not in the layer */
+  float* voxel_distance;   /* n: its ESDF distance, NaN when not observed / not in the layer */
+  float* distance;         /* n: trilinear ESDF distance */
+  float* gradient;         /* 3n: central differences of it */
+} ksg_esdf_query_out;
+int32_t ksg_query_esdf(ksg_integrator* h, int64_t n, const float* xyz_G, const ksg_esdf_query_out* out);
+int32_t ksg_query_esdf_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, const ksg_esdf_query_out* d_out, void* cuda_stream);
+
 /* Remove every block but keep the integrator: what Layer::removeAllBlocks() on both layers does to a live reference integrator.  The
  * fast integrator's two per-scan approximate sets (members of the integrator, fast.h:114-130) keep their contents and offsets, so the
  * next frame is integrated exactly as the reference integrator object would integrate it into its emptied layers.  Used by the

@@ -105,6 +105,24 @@ class KsgQueryOut(C.Structure):
     _fields_ = [(name, C.c_void_p) for name in QUERY_FIELDS]
 
 
+ESDF_QUERY_FIELDS = ("flags", "voxel_flags", "voxel_distance", "distance", "gradient")
+
+
+class KsgEsdfQueryOut(C.Structure):
+    """Mirror of `struct ksg_esdf_query_out` (include/ksg.h): one pointer per output, NULL = not wanted."""
+    _fields_ = [(name, C.c_void_p) for name in ESDF_QUERY_FIELDS]
+
+
+class KsgEsdfStats(C.Structure):
+    """Mirror of `struct ksg_esdf_stats` (include/ksg.h): what one ksg_update_esdf recomputed."""
+    _fields_ = [("blocks", C.c_int64), ("full", C.c_int64), ("changed_blocks", C.c_int64), ("site_blocks", C.c_int64),
+                ("site_changed", C.c_int64), ("x_blocks", C.c_int64), ("y_blocks", C.c_int64), ("z_blocks", C.c_int64),
+                ("reserved", C.c_int64 * 4)]
+
+    def as_dict(self) -> Dict[str, int]:
+        return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
+
+
 RENDER_FIELDS = ("depth", "points_G") + QUERY_FIELDS
 
 
@@ -295,6 +313,14 @@ def load_library(path: Optional[str] = None):
     lib.ksg_render_view_device.restype = C.c_int32
     lib.ksg_compute_esdf.argtypes = [H, C.c_float, C.c_float, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.ksg_compute_esdf.restype = C.c_int32
+    lib.ksg_update_esdf.argtypes = [H, C.c_float, C.c_float, C.POINTER(KsgEsdfStats)]
+    lib.ksg_update_esdf.restype = C.c_int32
+    lib.ksg_export_esdf.argtypes = [H, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.ksg_export_esdf.restype = C.c_int32
+    lib.ksg_query_esdf.argtypes = [H, C.c_int64, C.c_void_p, C.POINTER(KsgEsdfQueryOut)]
+    lib.ksg_query_esdf.restype = C.c_int32
+    lib.ksg_query_esdf_device.argtypes = [H, C.c_int64, C.c_void_p, C.POINTER(KsgEsdfQueryOut), C.c_void_p]
+    lib.ksg_query_esdf_device.restype = C.c_int32
     lib.ksg_clear_map.argtypes = [H]
     lib.ksg_clear_map.restype = C.c_int32
     lib.ksg_build_info.argtypes = []
@@ -311,7 +337,8 @@ KSG_SYMBOLS = ["ksg_default_config", "ksg_create", "ksg_destroy", "ksg_last_erro
                "ksg_unordered_map_schedule", "ksg_integrate_depth_k64", "ksg_integrate_depth_device_k64",
                "ksg_debug_chain_sum", "ksg_debug_tsdf_batch", "ksg_debug_apply_routes", "ksg_debug_fast_timeline", "ksg_integrate_depth_async", "ksg_wait_frame",
                "ksg_device_map_view", "ksg_merge_blocks_device", "ksg_copy_map_device", "ksg_integrate_image", "ksg_set_update_log", "ksg_fetch_update_log", "ksg_evaluate_labels", "ksg_extract_mesh", "ksg_clear_map", "ksg_copy_update_log_device", "ksg_merge_voxels_device",
-               "ksg_query_points", "ksg_query_points_device", "ksg_render_view", "ksg_render_view_device", "ksg_compute_esdf"]
+               "ksg_query_points", "ksg_query_points_device", "ksg_render_view", "ksg_render_view_device", "ksg_compute_esdf",
+               "ksg_update_esdf", "ksg_export_esdf", "ksg_query_esdf", "ksg_query_esdf_device"]
 
 
 def debug_chain_sum(terms: np.ndarray, s0: float, lib=None) -> np.float32:
@@ -665,6 +692,40 @@ class Integrator:
         self._check(self.lib.ksg_compute_esdf(self.handle, min_weight, max_distance, nb, *(C.c_void_p(a.ctypes.data) for a in out.values())),
                     "ksg_compute_esdf")
         return out
+
+    def update_esdf(self, max_distance: float, min_weight: float = 1e-4) -> Dict[str, int]:
+        """Bring the device ESDF layer up to date with the map (ksg_update_esdf); returns its stats (KsgEsdfStats fields)."""
+        st = KsgEsdfStats()
+        self._check(self.lib.ksg_update_esdf(self.handle, min_weight, max_distance, C.byref(st)), "ksg_update_esdf")
+        return st.as_dict()
+
+    def export_esdf(self, changed_only: bool = False) -> Dict[str, np.ndarray]:
+        """The device ESDF layer as of the last update (ksg_export_esdf): dict(block_index [n, 3] i32 in (z, y, x) order, distance [n, V]
+        f32, flags [n, V] u8) of every block it covers, or with changed_only of the blocks the last update rewrote."""
+        n = C.c_int64()
+        self._check(self.lib.ksg_export_esdf(self.handle, int(changed_only), 0, C.byref(n), None, None, None), "ksg_export_esdf")
+        nb, V = int(n.value), self.cfg.voxels_per_side ** 3
+        out = {"block_index": np.zeros((nb, 3), np.int32), "distance": np.zeros((nb, V), np.float32), "flags": np.zeros((nb, V), np.uint8)}
+        self._check(self.lib.ksg_export_esdf(self.handle, int(changed_only), nb, C.byref(n), *(C.c_void_p(a.ctypes.data) for a in out.values())),
+                    "ksg_export_esdf")
+        return out
+
+    def query_esdf(self, xyz) -> Dict[str, np.ndarray]:
+        """Point queries on the device ESDF layer (ksg_query_esdf): dict(flags [n] u8 (KSG_QUERY_*), voxel_flags [n] u8 (KSG_ESDF_*),
+        voxel_distance [n] f32, distance [n] f32 trilinear, gradient [n, 3] f32).  Invalid entries are NaN / 0, see include/ksg.h."""
+        p = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+        n = len(p)
+        out = {"flags": np.zeros(n, np.uint8), "voxel_flags": np.zeros(n, np.uint8), "voxel_distance": np.zeros(n, np.float32),
+               "distance": np.zeros(n, np.float32), "gradient": np.zeros((n, 3), np.float32)}
+        q = KsgEsdfQueryOut(**{k: v.ctypes.data for k, v in out.items()})
+        self._check(self.lib.ksg_query_esdf(self.handle, n, p.ctypes.data, C.byref(q)), "ksg_query_esdf")
+        return out
+
+    def query_esdf_device(self, d_xyz: int, n: int, out_ptrs: Dict[str, int], stream: int = 0):
+        """Enqueue ksg_query_esdf_device on `stream` (0 = the integrator's own stream): d_xyz and the values of out_ptrs (keys of
+        ESDF_QUERY_FIELDS; missing keys = not wanted) are raw device pointers.  Returns without waiting."""
+        q = KsgEsdfQueryOut(**{k: int(v) for k, v in out_ptrs.items() if v})
+        self._check(self.lib.ksg_query_esdf_device(self.handle, n, C.c_void_p(d_xyz), C.byref(q), C.c_void_p(stream)), "ksg_query_esdf_device")
 
     def query_points(self, xyz, min_weight: float = 1e-4, priors: bool = True) -> Dict[str, np.ndarray]:
         """Point queries on the device map (ksg_query_points): dict(flags [n] u8 (KSG_QUERY_*), tsdf_distance / tsdf_weight [n] f32,

@@ -63,6 +63,20 @@ class GpuIntegratorCore {
   // block per allocated map block: observed = OBSERVED, fixed = SURFACE, distance as computed; an unobserved voxel is voxblox's default
   // EsdfVoxel (distance 0, not observed).
   bool computeEsdf(float min_weight, float max_distance, vxb::Layer<vxb::EsdfVoxel>* esdf_layer);
+  // The ESDF kept on the device (ksg_update_esdf): brings the device layer up to date from the blocks that changed since the last call,
+  // then refreshes in *esdf_layer only the blocks that update rewrote (ksg_export_esdf changed_only), allocating new ones - after a full
+  // update (first call, new parameters, after a clear / reset / import, or after a call that failed) the whole layer.  Afterwards
+  // *esdf_layer holds what computeEsdf would give, provided only this call wrote it.  Works in kLazy mode without syncLayers().
+  bool updateEsdf(float min_weight, float max_distance, vxb::Layer<vxb::EsdfVoxel>* esdf_layer);
+  // ESDF point queries on the device layer as of the last updateEsdf (ksg_query_esdf): per point the KSG_QUERY_* flags, the containing
+  // voxel's KSG_ESDF_* flags and distance, the trilinear ESDF distance and its gradient.
+  struct EsdfQueryResult {
+    std::vector<uint8_t> flags, voxel_flags;   // n, n
+    std::vector<float> voxel_distance;         // n
+    std::vector<float> distance;               // n
+    std::vector<float> gradient;               // 3n
+  };
+  bool queryEsdf(const vxb::Pointcloud& points_G, EsdfQueryResult* result);
   int64_t lastVoxelUpdates() const { return last_voxel_updates_; }
   ksg_integrator* handle() { return handle_; }
 
@@ -70,6 +84,7 @@ class GpuIntegratorCore {
   void copyBlocks(const std::vector<int32_t>& idx);
   void syncAfterCall();        // eager mode: update log (fast) or updated blocks (merged)
   bool update_log_tried_ = false, update_log_on_ = false;
+  bool esdf_resync_ = true;    // updateEsdf: the host layer must be refreshed whole (first call, or the last call failed)
   ksg_integrator* handle_ = nullptr;
   vxb::Layer<vxb::TsdfVoxel>* tsdf_layer_;
   vxb::Layer<SemanticVoxel>* semantic_layer_;

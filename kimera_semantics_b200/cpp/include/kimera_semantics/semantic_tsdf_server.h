@@ -120,6 +120,12 @@ class SemanticTsdfServer {
   bool updateEsdfBatch(vxb::Layer<vxb::EsdfVoxel>* esdf_layer, float max_distance, float min_weight = 1e-4f) {
     return gpu().computeEsdf(min_weight, max_distance, esdf_layer);
   }
+  // voxblox's EsdfServer::updateEsdf: brings *esdf_layer up to date with the map, recomputing on the device only what the blocks changed
+  // since the last call can have changed (GpuIntegratorCore::updateEsdf); the same field as updateEsdfBatch, and like it needs no
+  // updateLayers().
+  bool updateEsdf(vxb::Layer<vxb::EsdfVoxel>* esdf_layer, float max_distance, float min_weight = 1e-4f) {
+    return gpu().updateEsdf(min_weight, max_distance, esdf_layer);
+  }
 
   vxb::Layer<vxb::TsdfVoxel>* getTsdfLayerPtr() { return tsdf_layer_.get(); }
   vxb::Layer<SemanticVoxel>* getSemanticLayerPtr() { return semantic_layer_.get(); }

@@ -348,6 +348,22 @@ bool GpuIntegratorCore::renderView(const vxb::Transformation& T_G_C, const doubl
   return ksg_render_view(handle_, T, K, w, h, min_depth, max_depth, min_weight, &out) == KSG_OK;
 }
 
+namespace {
+// one ESDF block from rows of ksg_compute_esdf / ksg_export_esdf: observed = OBSERVED, fixed = SURFACE; every other voxel is voxblox's
+// default EsdfVoxel
+void fillEsdfBlock(vxb::Block<vxb::EsdfVoxel>* blk, size_t V, const float* distance, const uint8_t* flags) {
+  blk->has_data() = true;
+  for (size_t v = 0; v < V; ++v) {
+    vxb::EsdfVoxel& e = blk->getVoxelByLinearIndex(v);
+    e = vxb::EsdfVoxel();
+    if (!(flags[v] & KSG_ESDF_OBSERVED)) continue;
+    e.distance = distance[v];
+    e.observed = true;
+    e.fixed = (flags[v] & KSG_ESDF_SURFACE) != 0;
+  }
+}
+}  // namespace
+
 bool GpuIntegratorCore::computeEsdf(float min_weight, float max_distance, vxb::Layer<vxb::EsdfVoxel>* esdf) {
   if (!esdf || esdf->voxels_per_side() != tsdf_layer_->voxels_per_side()) return false;
   const int64_t nb = ksg_num_blocks(handle_);
@@ -357,19 +373,46 @@ bool GpuIntegratorCore::computeEsdf(float min_weight, float max_distance, vxb::L
   std::vector<uint8_t> flags((size_t)nb * V);
   if (ksg_compute_esdf(handle_, min_weight, max_distance, nb, index.data(), distance.data(), flags.data()) != KSG_OK) return false;
   esdf->removeAllBlocks();
-  for (int64_t b = 0; b < nb; ++b) {
-    vxb::Block<vxb::EsdfVoxel>::Ptr blk = esdf->allocateNewBlock(vxb::BlockIndex(index[3 * b], index[3 * b + 1], index[3 * b + 2]));
-    blk->has_data() = true;
-    for (size_t v = 0; v < V; ++v) {
-      const uint8_t f = flags[b * V + v];
-      if (!(f & KSG_ESDF_OBSERVED)) continue;
-      vxb::EsdfVoxel& e = blk->getVoxelByLinearIndex(v);
-      e.distance = distance[b * V + v];
-      e.observed = true;
-      e.fixed = (f & KSG_ESDF_SURFACE) != 0;
-    }
-  }
+  for (int64_t b = 0; b < nb; ++b)
+    fillEsdfBlock(esdf->allocateNewBlock(vxb::BlockIndex(index[3 * b], index[3 * b + 1], index[3 * b + 2])).get(), V,
+                  distance.data() + b * V, flags.data() + b * V);
   return true;
+}
+
+bool GpuIntegratorCore::updateEsdf(float min_weight, float max_distance, vxb::Layer<vxb::EsdfVoxel>* esdf) {
+  if (!esdf || esdf->voxels_per_side() != tsdf_layer_->voxels_per_side()) return false;
+  // a call that fails leaves the host layer behind the device layer: the next one refreshes every block
+  const bool whole = esdf_resync_;
+  esdf_resync_ = true;
+  ksg_esdf_stats st;
+  if (ksg_update_esdf(handle_, min_weight, max_distance, &st) != KSG_OK) return false;
+  const int32_t changed_only = (st.full || whole) ? 0 : 1;
+  int64_t n = 0;
+  if (ksg_export_esdf(handle_, changed_only, 0, &n, nullptr, nullptr, nullptr) != KSG_OK) return false;
+  const size_t V = esdf->voxels_per_side() * esdf->voxels_per_side() * esdf->voxels_per_side();
+  std::vector<int32_t> index(3 * (size_t)n);
+  std::vector<float> distance((size_t)n * V);
+  std::vector<uint8_t> flags((size_t)n * V);
+  if (n > 0 && ksg_export_esdf(handle_, changed_only, n, &n, index.data(), distance.data(), flags.data()) != KSG_OK) return false;
+  // a refresh of every block starts the host layer over, as computeEsdf's does (after a clear or reset blocks may have gone)
+  if (!changed_only) esdf->removeAllBlocks();
+  for (int64_t b = 0; b < n; ++b)
+    fillEsdfBlock(esdf->allocateBlockPtrByIndex(vxb::BlockIndex(index[3 * b], index[3 * b + 1], index[3 * b + 2])).get(), V,
+                  distance.data() + b * V, flags.data() + b * V);
+  esdf_resync_ = false;
+  return true;
+}
+
+bool GpuIntegratorCore::queryEsdf(const vxb::Pointcloud& points_G, EsdfQueryResult* r) {
+  if (!r) return false;
+  const size_t n = points_G.size();
+  r->flags.assign(n, 0);
+  r->voxel_flags.assign(n, 0);
+  r->voxel_distance.assign(n, 0.0f);
+  r->distance.assign(n, 0.0f);
+  r->gradient.assign(3 * n, 0.0f);
+  ksg_esdf_query_out out = {r->flags.data(), r->voxel_flags.data(), r->voxel_distance.data(), r->distance.data(), r->gradient.data()};
+  return ksg_query_esdf(handle_, (int64_t)n, n ? reinterpret_cast<const float*>(points_G.data()) : nullptr, &out) == KSG_OK;
 }
 
 void GpuIntegratorCore::uploadLayers() {

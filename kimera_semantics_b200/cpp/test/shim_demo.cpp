@@ -1,7 +1,7 @@
 // Drives the drop-in C++ API exactly the way SemanticTsdfServer does (kimera_semantics_ros/src/semantic_tsdf_server.cpp:58-79):
 // build both layers, SemanticTsdfIntegratorFactory::create(method, ...), then integratePointCloud per frame.
 //   shim_demo <fast|merged|bogus> <frames.bin> <out.bin> [lazy] [--load ckpt] [--save ckpt] [--skip N] [--query in out] [--render in out]
-//             [--esdf max_distance out]
+//             [--esdf max_distance out] [--esdf-every N max_distance out]
 //     --load: SemanticTsdfServer::loadMap before the first frame; --save: saveMap after the last; --skip: ignore the first N frames
 //     --depth file: instead of the clouds of frames.bin (whose frame count must then be 0) feed depth + label frames:
 //              int32 n, int32 width, int32 height, double K[4], then per frame float T[7], float depth[w*h], uint8 label[w*h]
@@ -14,6 +14,8 @@
 //              arrays of --query's output for the n = w * h hit points
 //     --esdf max_distance out: after the last frame (also before any layer sync) SemanticTsdfServer::updateEsdfBatch (min_weight 1e-4),
 //              then vxblx_io::saveEsdfLayer to `out` - the reference driver's last step (kimera_semantics_rosbag.cpp:160-166)
+//     --esdf-every N max_distance out: SemanticTsdfServer::updateEsdf (min_weight 1e-4) into one host layer after every N-th frame of
+//              frames.bin and after the last, then vxblx_io::saveEsdfLayer of that layer to `out`
 // frames.bin : int32 n_frames, float voxel_size, int32 vps, int32 n_palette, palette n*(r,g,b,a,id), int32 n_dynamic, ids...,
 //              then per frame: int32 n, float T[7], float xyz[3n], uint8 rgba[4n]
 // out.bin    : int32 n_blocks, then per block (sorted z,y,x): int32 idx[3], per voxel: float d, float w, u8 rgba[4], u8 label,
@@ -53,8 +55,9 @@ int main(int argc, char** argv) {
   bool lazy = false;
   const char *load_path = nullptr, *save_path = nullptr, *depth_path = nullptr, *query_in = nullptr, *query_out = nullptr;
   const char *render_in = nullptr, *render_out = nullptr, *esdf_out = nullptr;
-  float esdf_max_distance = 0.0f;
-  int skip = 0;
+  float esdf_max_distance = 0.0f, inc_max_distance = 0.0f;
+  const char* inc_out = nullptr;
+  int skip = 0, esdf_every = 0;
   for (int a = 4; a < argc; ++a) {
     if (std::strcmp(argv[a], "lazy") == 0) lazy = true;
     else if (std::strcmp(argv[a], "--load") == 0 && a + 1 < argc) load_path = argv[++a];
@@ -64,6 +67,11 @@ int main(int argc, char** argv) {
     else if (std::strcmp(argv[a], "--query") == 0 && a + 2 < argc) { query_in = argv[++a]; query_out = argv[++a]; }
     else if (std::strcmp(argv[a], "--render") == 0 && a + 2 < argc) { render_in = argv[++a]; render_out = argv[++a]; }
     else if (std::strcmp(argv[a], "--esdf") == 0 && a + 2 < argc) { esdf_max_distance = (float)std::atof(argv[++a]); esdf_out = argv[++a]; }
+    else if (std::strcmp(argv[a], "--esdf-every") == 0 && a + 3 < argc) {
+      esdf_every = std::max(1, std::atoi(argv[++a]));
+      inc_max_distance = (float)std::atof(argv[++a]);
+      inc_out = argv[++a];
+    }
   }
   SemanticTsdfServer::Params params;
   params.tsdf_voxel_size = voxel_size;
@@ -75,6 +83,8 @@ int main(int argc, char** argv) {
   vxb::Layer<SemanticVoxel>& semantic_layer = *server.getSemanticLayerPtr();
   GpuIntegratorCore* core = &server.gpu();
   if (load_path) KSG_CHECK(server.loadMap(load_path)) << "cannot load " << load_path;
+  vxb::Layer<vxb::EsdfVoxel> inc(tsdf_layer.voxel_size(), tsdf_layer.voxels_per_side());
+  int inc_updates = 0;
   for (int fr = 0; fr < n_frames; ++fr) {
     const int n = rd<int32_t>(f);
     float T[7]; f.read(reinterpret_cast<char*>(T), sizeof(T));
@@ -85,6 +95,16 @@ int main(int argc, char** argv) {
     server.processPointCloud(vxb::Transformation(T[0], T[1], T[2], T[3], vxb::Point(T[4], T[5], T[6])), pts, cols, /*stamp=*/0.2 * fr);
     std::printf("frame %d: %d points, %lld voxel updates, %zu blocks in the host layer\n", fr, n, (long long)core->lastVoxelUpdates(),
                 tsdf_layer.getNumberOfAllocatedBlocks());
+    if (inc_out && (fr + 1) % esdf_every == 0) {
+      KSG_CHECK(server.updateEsdf(&inc, inc_max_distance)) << "esdf update failed";
+      ++inc_updates;
+    }
+  }
+  if (inc_out) {
+    KSG_CHECK(server.updateEsdf(&inc, inc_max_distance)) << "esdf update failed";
+    KSG_CHECK(vxblx_io::saveEsdfLayer(inc_out, inc)) << "cannot save " << inc_out;
+    std::printf("esdf-every: %d updates, %zu blocks%s\n", inc_updates + 1, inc.getNumberOfAllocatedBlocks(),
+                lazy ? " (host layers not synchronised)" : "");
   }
   if (depth_path) {
     std::ifstream df(depth_path, std::ios::binary);

@@ -14,6 +14,7 @@
 #include <string>
 #include <type_traits>
 #include <unordered_map>
+#include <unordered_set>
 #include <utility>
 #include <vector>
 
@@ -331,6 +332,18 @@ struct ksg_integrator {
   int deep_threads = 0;
   int short_t_ctas = 0;
 
+  // device ESDF layer (ksg_update_esdf, ksg_esdf.cuh): rows by pool slot, max_blocks of them, allocated by the first update
+  float* esdf_dist = nullptr;
+  uint8_t *esdf_flags = nullptr, *esdf_site = nullptr;
+  bool esdf_full = true;              // the next update recomputes everything: no update yet, or a clear / reset / import since the last
+  bool esdf_valid = false;            // the layer describes slots [0, esdf_blocks) of the map (export and query allowed)
+  float esdf_min_weight = 0.0f, esdf_max_distance = 0.0f;
+  int esdf_stamp = 0;                 // frame_stamp at the last update: blocks stamped after it changed
+  int64_t esdf_blocks = 0;
+  std::vector<uint64_t> esdf_keys;    // key of each slot of the layer
+  std::vector<uint8_t> esdf_has_site; // per slot: the row holds a site
+  std::vector<int> esdf_rewritten;    // slots whose output the last update rewrote, in (z, y, x) order
+
   long long* tile_debug = nullptr;  // optional per-tile (records, cycles) trace
   int apply_smem = 0;
   int apply_nch = 1;
@@ -418,6 +431,8 @@ int reset_map(ksg_integrator* h, cudaStream_t s) {
   h->last_blocks_touched = 0;
   h->deferred_status = 0;
   h->merged_log_count = 0;
+  h->esdf_full = true;
+  h->esdf_valid = false;
   KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
 }
@@ -1978,13 +1993,14 @@ int32_t ksg_render_view_device(ksg_integrator* h, const float* T_G_C_host, const
 
 namespace {
 // The work sets of the x and y passes and the neighbour tables of the three passes (ksg_esdf.cuh), from the keys of the allocated blocks
-// (output order) and which of them hold a site.  Blocks outside the key range hold no site, and neither does any block sharing their
+// (the site rows: the x pass table holds indices into alloc), which of them hold a site, and the z work set `out` (indices into alloc;
+// NULL: every allocated block, in alloc order).  Blocks outside the key range hold no site, and neither does any block sharing their
 // out-of-range coordinate, so their pass results are "none" and they are left out.
 struct EsdfWork {
   int64_t n_x = 0, n_y = 0;
   std::vector<int> tx, ty, tz;   // per block of the x / y / z pass: 2 Rb + 1 indices into the previous stage, -1 = none
 
-  void build(const std::vector<I3>& alloc, const std::vector<uint8_t>& has_site, int Rb) {
+  void build(const std::vector<I3>& alloc, const std::vector<uint8_t>& has_site, int Rb, const std::vector<int>* out = nullptr) {
     const int span = 2 * Rb + 1;
     auto moved = [](I3 b, int axis, int k) { if (axis == 0) b.x += k; else if (axis == 1) b.y += k; else b.z += k; return b; };
     std::unordered_map<uint64_t, int> site_at;      // site block -> its index in alloc
@@ -1997,10 +2013,14 @@ struct EsdfWork {
         if (key_in_range(b)) near_x[pack_key(b)] = 1;
       }
     }
-    // Y: within Rb along z of an allocated block, with a near_x block within Rb along y
+    std::vector<I3> zs;
+    if (out)
+      for (int a : *out) zs.push_back(alloc[a]);
+    const std::vector<I3>& z_blocks = out ? zs : alloc;
+    // Y: within Rb along z of a z block, with a near_x block within Rb along y
     std::unordered_map<uint64_t, int> y_at;         // -1: looked at and left out
     std::vector<I3> ys;
-    for (const I3& a : alloc)
+    for (const I3& a : z_blocks)
       for (int k = -Rb; k <= Rb; ++k) {
         const I3 b = moved(a, 2, k);
         if (!key_in_range(b) || y_at.count(pack_key(b))) continue;
@@ -2036,7 +2056,7 @@ struct EsdfWork {
     };
     table(xs, 0, site_at, &tx);
     table(ys, 1, x_at, &ty);
-    table(alloc, 2, y_at, &tz);
+    table(z_blocks, 2, y_at, &tz);
   }
 };
 
@@ -2044,16 +2064,24 @@ int esdf_grid(ksg_integrator* h, int64_t blocks) {
   const int64_t items = blocks * (int64_t)h->dc.vps * h->dc.vps * h->dc.vps;
   return (int)std::max<int64_t>(1, std::min<int64_t>((items + kEsdfThreads - 1) / kEsdfThreads, (int64_t)h->sm_count * 16));
 }
-}  // namespace
 
-int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance, int64_t capacity_blocks, int32_t* block_index,
-                         float* distance, uint8_t* flags) {
+// the checks of ksg_compute_esdf and ksg_update_esdf; *W = the window
+int esdf_args(ksg_integrator* h, float min_weight, float max_distance, int* W) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
   if (!(min_weight >= 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: NaN or negative min_weight");
   if (!std::isfinite(max_distance) || !(max_distance > 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: max_distance must be finite and > 0");
   const double Wd = std::ceil((double)max_distance / (double)h->dc.voxel_size) + 1.0;
   if (!(Wd <= (double)kEsdfMaxWindow)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: ceil(max_distance / voxel_size) + 1 > 512");
   if (h->dc.shard_count > 1) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: a sharded integrator holds only its own tiles");
+  *W = (int)Wd;
+  return KSG_OK;
+}
+}  // namespace
+
+int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance, int64_t capacity_blocks, int32_t* block_index,
+                         float* distance, uint8_t* flags) {
+  int W = 0;
+  { const int rca = esdf_args(h, min_weight, max_distance, &W); if (rca) return rca; }
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
@@ -2065,7 +2093,7 @@ int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance
   { const int rco = slots_zyx(h, &order, index.data()); if (rco) return rco; }
   if (block_index) std::memcpy(block_index, index.data(), sizeof(int32_t) * 3 * nb);
   if (!distance && !flags) return KSG_OK;
-  const int W = (int)Wd, vps = h->dc.vps, Rb = (W + vps - 1) / vps;
+  const int vps = h->dc.vps, Rb = (W + vps - 1) / vps;
   const size_t V = (size_t)vps * vps * vps;
   Resources tmp;
   int* d_slots = nullptr; uint8_t* d_site = nullptr; uint8_t* d_has = nullptr;
@@ -2076,7 +2104,7 @@ int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance
   KSG_CUDA(cudaMemcpyAsync(d_slots, order.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s));
   ++h->n_launches;
   k_esdf_sites<<<(int)std::min<int64_t>(nb, (int64_t)h->sm_count * 8), kEsdfThreads, 0, s>>>(h->dc, h->map, d_slots, (int)nb, min_weight,
-                                                                                              d_site, d_has);
+                                                                                              0, d_site, d_has, nullptr);
   std::vector<uint8_t> has((size_t)nb);
   KSG_CUDA(cudaMemcpyAsync(has.data(), d_has, nb, cudaMemcpyDeviceToHost, s));
   KSG_CUDA(cudaStreamSynchronize(s));
@@ -2107,6 +2135,252 @@ int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance
   if (distance) KSG_CUDA(cudaMemcpyAsync(distance, d_dist, sizeof(float) * nb * V, cudaMemcpyDeviceToHost, s));
   if (flags) KSG_CUDA(cudaMemcpyAsync(flags, d_flags, nb * V, cudaMemcpyDeviceToHost, s));
   KSG_CUDA(cudaStreamSynchronize(s));
+  return KSG_OK;
+}
+
+int32_t ksg_update_esdf(ksg_integrator* h, float min_weight, float max_distance, ksg_esdf_stats* stats) {
+  int W = 0;
+  { const int rca = esdf_args(h, min_weight, max_distance, &W); if (rca) return rca; }
+  KSG_CUDA(cudaSetDevice(h->device));
+  KSG_CUDA(cudaDeviceSynchronize());
+  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  const int vps = h->dc.vps, Rb = (W + vps - 1) / vps;
+  const size_t V = (size_t)vps * vps * vps;
+  const int64_t nb = h->num_blocks;
+  const bool full = h->esdf_full || min_weight != h->esdf_min_weight || max_distance != h->esdf_max_distance;
+  // Until this call succeeds the layer is not trusted: the site bytes are rewritten in place before the passes run, so a call that
+  // fails part-way would leave bytes that no longer differ from the map while their outputs are stale.  The next call is then full,
+  // and export and query are refused until it succeeds.
+  h->esdf_full = true;
+  h->esdf_valid = false;
+  const size_t rows = (size_t)h->map.max_blocks;
+  if (!h->esdf_dist) KSG_CUDA(h->res.device(&h->esdf_dist, rows * V));
+  if (!h->esdf_flags) KSG_CUDA(h->res.device(&h->esdf_flags, rows * V));
+  if (!h->esdf_site) KSG_CUDA(h->res.device(&h->esdf_site, rows * V));
+  if (h->esdf_has_site.size() != rows) h->esdf_has_site.assign(rows, 0);
+  const int64_t prev = full ? 0 : h->esdf_blocks;   // rows below prev hold the sites and outputs of the last update
+  cudaStream_t s = h->own_stream;
+  std::vector<uint64_t> keys((size_t)nb);
+  if (nb > 0) KSG_CUDA(cudaMemcpy(keys.data(), h->map.slot_key, sizeof(uint64_t) * nb, cudaMemcpyDeviceToHost));
+  // C: the slots stamped after the last update, and the slots allocated since
+  std::vector<uint8_t> in_c((size_t)nb, 0);
+  for (int64_t i = prev; i < nb; ++i) in_c[i] = 1;
+  if (prev > 0) {
+    std::vector<int> pos_slot(h->ht_cap), pos_stamp(h->ht_cap);
+    KSG_CUDA(cudaMemcpy(pos_slot.data(), h->map.ht_slot, sizeof(int) * h->ht_cap, cudaMemcpyDeviceToHost));
+    KSG_CUDA(cudaMemcpy(pos_stamp.data(), h->map.touched_stamp, sizeof(int) * h->ht_cap, cudaMemcpyDeviceToHost));
+    for (uint32_t p = 0; p < h->ht_cap; ++p)
+      if (pos_slot[p] >= 0 && pos_slot[p] < nb && pos_stamp[p] > h->esdf_stamp) in_c[pos_slot[p]] = 1;
+  }
+  std::unordered_map<uint64_t, int> slot_of;
+  slot_of.reserve((size_t)nb);
+  for (int64_t i = 0; i < nb; ++i) slot_of[keys[i]] = (int)i;
+  auto find = [&](I3 b) { if (!key_in_range(b)) return -1; const auto it = slot_of.find(pack_key(b)); return it == slot_of.end() ? -1 : it->second; };
+  // R: C and its allocated face neighbours, whose site bytes are recomputed
+  std::vector<uint8_t> in_r(in_c);
+  int64_t n_c = 0;
+  for (int64_t i = 0; i < nb; ++i) {
+    if (!in_c[i]) continue;
+    ++n_c;
+    const I3 b = unpack_key(keys[i]);
+    for (int k = 0; k < 6; ++k) {
+      I3 nbk = b;
+      const int d = (k & 1) ? 1 : -1;
+      if (k < 2) nbk.x += d; else if (k < 4) nbk.y += d; else nbk.z += d;
+      const int j = find(nbk);
+      if (j >= 0) in_r[j] = 1;
+    }
+  }
+  std::vector<int> r_slots;
+  for (int64_t i = 0; i < nb; ++i) if (in_r[i]) r_slots.push_back((int)i);
+  ksg_esdf_stats st{};
+  st.blocks = nb;
+  st.full = full ? 1 : 0;
+  st.changed_blocks = n_c;
+  st.site_blocks = (int64_t)r_slots.size();
+  std::vector<int> d_list;
+  if (!r_slots.empty()) {
+    const int64_t nr = (int64_t)r_slots.size();
+    Resources tmp;
+    int* d_r = nullptr; uint8_t* d_has = nullptr;
+    KSG_CUDA(tmp.device(&d_r, nr));
+    KSG_CUDA(tmp.device(&d_has, 2 * nr));   // has_site, then changed
+    // rows new to the layer held no site before
+    if (nb > prev) KSG_CUDA(cudaMemsetAsync(h->esdf_site + (size_t)prev * V, 0, (size_t)(nb - prev) * V, s));
+    KSG_CUDA(cudaMemcpyAsync(d_r, r_slots.data(), sizeof(int) * nr, cudaMemcpyHostToDevice, s));
+    ++h->n_launches;
+    k_esdf_sites<<<(int)std::min<int64_t>(nr, (int64_t)h->sm_count * 8), kEsdfThreads, 0, s>>>(h->dc, h->map, d_r, (int)nr, min_weight, 1,
+                                                                                                h->esdf_site, d_has, d_has + nr);
+    std::vector<uint8_t> has((size_t)(2 * nr));
+    KSG_CUDA(cudaMemcpyAsync(has.data(), d_has, 2 * nr, cudaMemcpyDeviceToHost, s));
+    KSG_CUDA(cudaStreamSynchronize(s));
+    KSG_CUDA(cudaGetLastError());
+    // S: the recomputed blocks whose site bytes changed; D = C + the allocated blocks within Rb (Chebyshev) of S, by a separable dilation
+    // clamped to the allocated blocks' bounding box (an intermediate key takes the x, then the y coordinate of the allocated block it
+    // reaches, so nothing outside the box is needed): the sets stay within |S| (2Rb + 1)^2 and the box, whatever the window
+    I3 lo = unpack_key(keys[0]), hi = lo;
+    for (int64_t i = 1; i < nb; ++i) {
+      const I3 b = unpack_key(keys[i]);
+      lo.x = std::min(lo.x, b.x); lo.y = std::min(lo.y, b.y); lo.z = std::min(lo.z, b.z);
+      hi.x = std::max(hi.x, b.x); hi.y = std::max(hi.y, b.y); hi.z = std::max(hi.z, b.z);
+    }
+    std::unordered_set<uint64_t> sx, sxy;
+    for (int64_t r = 0; r < nr; ++r) {
+      h->esdf_has_site[r_slots[r]] = has[r];
+      if (!has[nr + r]) continue;
+      ++st.site_changed;
+      const I3 b = unpack_key(keys[r_slots[r]]);
+      for (int x = std::max(lo.x, b.x - Rb); x <= std::min(hi.x, b.x + Rb); ++x) { I3 c = b; c.x = x; sx.insert(pack_key(c)); }
+    }
+    for (uint64_t kx : sx) {
+      const I3 b = unpack_key(kx);
+      for (int y = std::max(lo.y, b.y - Rb); y <= std::min(hi.y, b.y + Rb); ++y) { I3 c = b; c.y = y; sxy.insert(pack_key(c)); }
+    }
+    for (int64_t i = 0; i < nb; ++i) {
+      bool dirty = in_c[i];
+      const I3 b = unpack_key(keys[i]);
+      for (int z = std::max(lo.z, b.z - Rb); z <= std::min(hi.z, b.z + Rb) && !dirty && !sxy.empty(); ++z) {
+        I3 c = b; c.z = z; dirty = sxy.count(pack_key(c)) > 0;
+      }
+      if (dirty) d_list.push_back((int)i);
+    }
+    std::sort(d_list.begin(), d_list.end(), [&](int a, int b) { return keys[a] < keys[b]; });
+    // the passes over D, reading the stored site bytes of the whole map
+    std::vector<I3> alloc((size_t)nb);
+    for (int64_t i = 0; i < nb; ++i) alloc[i] = unpack_key(keys[i]);
+    EsdfWork wk;
+    wk.build(alloc, h->esdf_has_site, Rb, &d_list);
+    const int64_t nd = (int64_t)d_list.size();
+    st.x_blocks = wk.n_x;
+    st.y_blocks = wk.n_y;
+    st.z_blocks = nd;
+    int *d_tx = nullptr, *d_ty = nullptr, *d_tz = nullptr, *d_a = nullptr, *d_b = nullptr, *d_d = nullptr;
+    KSG_CUDA(tmp.device(&d_tx, wk.tx.size()));
+    KSG_CUDA(tmp.device(&d_ty, wk.ty.size()));
+    KSG_CUDA(tmp.device(&d_tz, wk.tz.size()));
+    KSG_CUDA(tmp.device(&d_a, wk.n_x * V));
+    KSG_CUDA(tmp.device(&d_b, wk.n_y * V));
+    KSG_CUDA(tmp.device(&d_d, nd));
+    KSG_CUDA(cudaMemcpyAsync(d_tx, wk.tx.data(), sizeof(int) * wk.tx.size(), cudaMemcpyHostToDevice, s));
+    KSG_CUDA(cudaMemcpyAsync(d_ty, wk.ty.data(), sizeof(int) * wk.ty.size(), cudaMemcpyHostToDevice, s));
+    KSG_CUDA(cudaMemcpyAsync(d_tz, wk.tz.data(), sizeof(int) * wk.tz.size(), cudaMemcpyHostToDevice, s));
+    KSG_CUDA(cudaMemcpyAsync(d_d, d_list.data(), sizeof(int) * nd, cudaMemcpyHostToDevice, s));
+    const EsdfOut none{nullptr, nullptr, nullptr, 0.0f, 0.0f};
+    const EsdfOut eo{h->esdf_dist, h->esdf_flags, d_d, min_weight, max_distance};
+    h->n_launches += 3;
+    k_esdf_pass<0><<<esdf_grid(h, wk.n_x), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_x, W, Rb, d_tx, h->esdf_site, nullptr, d_a, nullptr, none);
+    k_esdf_pass<1><<<esdf_grid(h, wk.n_y), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_y, W, Rb, d_ty, nullptr, d_a, d_b, nullptr, none);
+    k_esdf_pass<2, true><<<esdf_grid(h, nd), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)nd, W, Rb, d_tz, nullptr, d_b, nullptr, h->esdf_site, eo);
+    KSG_CUDA(cudaGetLastError());
+    KSG_CUDA(cudaStreamSynchronize(s));
+  }
+  h->esdf_full = false;
+  h->esdf_valid = true;
+  h->esdf_min_weight = min_weight;
+  h->esdf_max_distance = max_distance;
+  h->esdf_stamp = h->frame_stamp;
+  h->esdf_blocks = nb;
+  h->esdf_keys = std::move(keys);
+  h->esdf_rewritten = std::move(d_list);
+  if (stats) *stats = st;
+  return KSG_OK;
+}
+
+int32_t ksg_export_esdf(ksg_integrator* h, int32_t changed_only, int64_t capacity_blocks, int64_t* n_blocks, int32_t* block_index,
+                        float* distance, uint8_t* flags) {
+  if (!h) return KSG_ERR_INVALID_ARGUMENT;
+  if (!h->esdf_valid) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf export: no ksg_update_esdf since the handle was created, cleared or reset");
+  std::vector<int> all;
+  if (!changed_only) {
+    all.resize((size_t)h->esdf_blocks);
+    for (int64_t i = 0; i < h->esdf_blocks; ++i) all[i] = (int)i;
+    std::sort(all.begin(), all.end(), [&](int a, int b) { return h->esdf_keys[a] < h->esdf_keys[b]; });
+  }
+  const std::vector<int>& list = changed_only ? h->esdf_rewritten : all;
+  const int64_t n = (int64_t)list.size();
+  if (n_blocks) *n_blocks = n;
+  if (!block_index && !distance && !flags) return KSG_OK;
+  if (n > capacity_blocks) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf export: block capacity too small (n_blocks holds the need)");
+  if (block_index) for (int64_t i = 0; i < n; ++i) put_block_index(block_index, i, h->esdf_keys[list[i]]);
+  if ((!distance && !flags) || n == 0) return KSG_OK;
+  KSG_CUDA(cudaSetDevice(h->device));
+  const size_t V = (size_t)h->dc.vps * h->dc.vps * h->dc.vps;
+  Resources tmp;
+  int* d_slots = nullptr; float* d_dist = nullptr; uint8_t* d_flags = nullptr;
+  KSG_CUDA(tmp.device(&d_slots, n));
+  if (distance) KSG_CUDA(tmp.device(&d_dist, n * V));
+  if (flags) KSG_CUDA(tmp.device(&d_flags, n * V));
+  cudaStream_t s = h->own_stream;
+  KSG_CUDA(cudaMemcpyAsync(d_slots, list.data(), sizeof(int) * n, cudaMemcpyHostToDevice, s));
+  ++h->n_launches;
+  k_esdf_gather<<<esdf_grid(h, n), kEsdfThreads, 0, s>>>((int)V, d_slots, (int)n, h->esdf_dist, h->esdf_flags, d_dist, d_flags);
+  KSG_CUDA(cudaGetLastError());
+  if (distance) KSG_CUDA(cudaMemcpyAsync(distance, d_dist, sizeof(float) * n * V, cudaMemcpyDeviceToHost, s));
+  if (flags) KSG_CUDA(cudaMemcpyAsync(flags, d_flags, n * V, cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
+  return KSG_OK;
+}
+
+namespace {
+// *work = false: nothing to compute (n = 0 or no output wanted)
+int esdf_query_args(ksg_integrator* h, int64_t n, const float* xyz, const ksg_esdf_query_out* o, bool* work) {
+  if (!h) return KSG_ERR_INVALID_ARGUMENT;
+  if (!o || n < 0) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf query: NULL out or n < 0");
+  if (n > 0 && !xyz) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf query: NULL points");
+  if (h->dc.shard_count > 1) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf query: a sharded integrator holds only its own tiles");
+  if (!h->esdf_valid) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf query: no ksg_update_esdf since the handle was created, cleared or reset");
+  *work = n > 0 && (o->flags || o->voxel_flags || o->voxel_distance || o->distance || o->gradient);
+  return KSG_OK;
+}
+void launch_esdf_query(ksg_integrator* h, int64_t n, const float* d_xyz, const ksg_esdf_query_out& o, cudaStream_t s) {
+  static_assert(sizeof(ksg_esdf_query_out) == sizeof(EsdfQueryOut), "ksg_esdf_query_out layout");
+  const EsdfQueryOut q{o.flags, o.voxel_flags, o.voxel_distance, o.distance, o.gradient};
+  const EsdfLayer layer{h->esdf_dist, h->esdf_flags, (int)h->esdf_blocks};
+  const int grid = (int)std::min<int64_t>((n + kQueryThreads - 1) / kQueryThreads, (int64_t)h->sm_count * 8);
+  ++h->n_launches;
+  k_query_esdf<<<grid, kQueryThreads, 0, s>>>(h->dc, h->map, layer, d_xyz, (long long)n, q, (o.flags || o.distance) ? 1 : 0,
+                                              (o.flags || o.gradient) ? 1 : 0);
+}
+}  // namespace
+
+int32_t ksg_query_esdf(ksg_integrator* h, int64_t n, const float* xyz_G, const ksg_esdf_query_out* out) {
+  bool work = false;
+  { const int rca = esdf_query_args(h, n, xyz_G, out, &work); if (rca) return rca; }
+  KSG_CUDA(cudaSetDevice(h->device));
+  KSG_CUDA(cudaDeviceSynchronize());
+  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  if (!work) return KSG_OK;
+  const ksg_esdf_query_out& o = *out;
+  const size_t N = (size_t)n;
+  // one device buffer: points, then every wanted output
+  const size_t sizes[6] = {12 * N, o.flags ? N : 0, o.voxel_flags ? N : 0, o.voxel_distance ? 4 * N : 0, o.distance ? 4 * N : 0,
+                           o.gradient ? 12 * N : 0};
+  size_t off[6], total = 0;
+  for (int k = 0; k < 6; ++k) { off[k] = total; total += (sizes[k] + 255) / 256 * 256; }
+  Resources tmp;
+  uint8_t* d = nullptr;
+  KSG_CUDA(tmp.device(&d, total));
+  auto at = [&](int k) -> void* { return sizes[k] ? (void*)(d + off[k]) : nullptr; };
+  const ksg_esdf_query_out dq{(uint8_t*)at(1), (uint8_t*)at(2), (float*)at(3), (float*)at(4), (float*)at(5)};
+  void* host[6] = {nullptr, o.flags, o.voxel_flags, o.voxel_distance, o.distance, o.gradient};
+  cudaStream_t s = h->own_stream;
+  KSG_CUDA(cudaMemcpyAsync(d, xyz_G, sizes[0], cudaMemcpyHostToDevice, s));
+  launch_esdf_query(h, n, (const float*)d, dq, s);
+  KSG_CUDA(cudaGetLastError());
+  for (int k = 1; k < 6; ++k)
+    if (sizes[k]) KSG_CUDA(cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
+  return KSG_OK;
+}
+
+int32_t ksg_query_esdf_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, const ksg_esdf_query_out* d_out, void* cuda_stream) {
+  bool work = false;
+  { const int rca = esdf_query_args(h, n, d_xyz_G, d_out, &work); if (rca) return rca; }
+  if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
+  if (!work) return KSG_OK;
+  KSG_CUDA(cudaSetDevice(h->device));
+  launch_esdf_query(h, n, d_xyz_G, *d_out, cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream);
+  KSG_CUDA(cudaGetLastError());
   return KSG_OK;
 }
 
@@ -2216,6 +2490,7 @@ int32_t ksg_import_blocks(ksg_integrator* h, int64_t n, const int32_t* block_ind
   KSG_CUDA(cudaSetDevice(h->device));
   KSG_CUDA(cudaDeviceSynchronize());
   { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  h->esdf_full = true;     // the import writes blocks without stamping them
   const DevCfg& dc = h->dc;
   HostBlockTable table;
   { const int rct = table.load(h); if (rct) return rct; }
@@ -2569,6 +2844,8 @@ int32_t ksg_clear_map(ksg_integrator* h) {
   KSG_CUDA(cudaMemsetAsync(&h->d_cnt->n_new_blocks, 0, sizeof(int), s));
   h->num_blocks = 0;
   h->last_blocks_touched = 0;
+  h->esdf_full = true;     // the stamps restart at 0 while frame_stamp does not, and the slots are reused
+  h->esdf_valid = false;
   KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
 }

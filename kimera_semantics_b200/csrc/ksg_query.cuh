@@ -70,20 +70,28 @@ __device__ __forceinline__ int query_block_slot(const MapRef& map, QueryBlocks& 
   return key_in_range(b) ? ht_lookup_slot(map, pack_key(b)) : -1;
 }
 
-// distance of voxel g if it is allocated and observed
-__device__ __forceinline__ bool query_corner(const DevCfg& cfg, const MapRef& map, QueryBlocks& w, I3 g, float min_weight, float& d) {
-  const int s = query_block_slot(map, w, block_of_voxel(g, cfg.vps_inv));
-  if (s < 0) return false;
-  const int vm = cfg.vps - 1;
-  int vox;
-  const uint8_t* chunk = mesh_voxel_chunk(cfg, map, s, g.x & vm, g.y & vm, g.z & vm, vox);
-  if (!(__ldg((const float*)(chunk + cfg.plane_f32) + vox) > min_weight)) return false;
-  d = __ldg((const float*)chunk + vox);
-  return true;
-}
+// Corner fetch of D(p): the distance of voxel g if it is allocated and observed.  query_interp_at and query_stencil take the corner
+// fetch as a parameter, so the ESDF query (ksg_esdf.cuh) runs the same arithmetic on its own layer.
+struct TsdfCorner {
+  const DevCfg& cfg;
+  const MapRef& map;
+  QueryBlocks& w;
+  float min_weight;
+  __device__ __forceinline__ bool operator()(I3 g, float& d) const {
+    const int s = query_block_slot(map, w, block_of_voxel(g, cfg.vps_inv));
+    if (s < 0) return false;
+    const int vm = cfg.vps - 1;
+    int vox;
+    const uint8_t* chunk = mesh_voxel_chunk(cfg, map, s, g.x & vm, g.y & vm, g.z & vm, vox);
+    if (!(__ldg((const float*)(chunk + cfg.plane_f32) + vox) > min_weight)) return false;
+    d = __ldg((const float*)chunk + vox);
+    return true;
+  }
+};
 
-// trilinear distance D(p); false when p is out of range or a corner is missing / unobserved
-__device__ __forceinline__ bool query_interp(const DevCfg& cfg, const MapRef& map, QueryBlocks& w, F3 p, float min_weight, float& out) {
+// trilinear distance D(p); false when p is out of range or corner(g, d) fails for one of the 8 corners
+template <class Corner>
+__device__ __forceinline__ bool query_interp_at(const DevCfg& cfg, const Corner& corner, F3 p, float& out) {
   if (!index_in_range(f3(p.x * cfg.vsi, p.y * cfg.vsi, p.z * cfg.vsi))) return false;
   const float vs = cfg.voxel_size;
   I3 g0 = grid_index(p, cfg.vsi);
@@ -98,7 +106,7 @@ __device__ __forceinline__ bool query_interp(const DevCfg& cfg, const MapRef& ma
   for (int i = 0; i < 8; ++i) {
     I3 c = g0;
     c.x += i >> 2; c.y += (i >> 1) & 1; c.z += i & 1;
-    if (!query_corner(cfg, map, w, c, min_weight, d[i])) return false;
+    if (!corner(c, d[i])) return false;
   }
   const float b0 = d[0];
   const float b1 = -d[0] + d[4];
@@ -110,6 +118,40 @@ __device__ __forceinline__ bool query_interp(const DevCfg& cfg, const MapRef& ma
   const float b7 = ((((((-d[0] + d[1]) + d[2]) - d[3]) + d[4]) - d[5]) - d[6]) + d[7];
   out = ((((((b0 + x * b1) + y * b2) + z * b3) + (x * y) * b4) + (y * z) * b5) + (z * x) * b6) + ((x * y) * z) * b7;
   return true;
+}
+
+// D(p) of the TSDF (k_render_view's march)
+__device__ __forceinline__ bool query_interp(const DevCfg& cfg, const MapRef& map, QueryBlocks& w, F3 p, float min_weight, float& out) {
+  return query_interp_at(cfg, TsdfCorner{cfg, map, w, min_weight}, p, out);
+}
+
+// D(p) when `interp` (the containing voxel is observed, so it can be valid) and the gradient when need_grad: sets INTERPOLATED /
+// GRADIENT in flags and writes the valid values.  Evaluation 0: D(p); 2a + 1 / 2a + 2: D(p + vs e_a) / D(p - vs e_a).  One loop (not
+// unrolled): the probe code is emitted once.
+template <class Corner>
+__device__ __forceinline__ void query_stencil(const DevCfg& cfg, const Corner& corner, F3 p, bool interp, int need_grad, int& flags,
+                                              float& dist, float& gx, float& gy, float& gz) {
+  const float vs = cfg.voxel_size;
+  float dplus = 0.0f, ga[3] = {0.0f, 0.0f, 0.0f};
+  const int e_first = interp ? 0 : 1;
+  const int e_end = need_grad ? 7 : 1;
+#pragma unroll 1
+  for (int e = e_first; e < e_end; ++e) {
+    const int a = (e - 1) >> 1;
+    const float off = (e & 1) ? vs : -vs;
+    const F3 pe = f3(a == 0 ? p.x + off : p.x, a == 1 ? p.y + off : p.y, a == 2 ? p.z + off : p.z);
+    float v;
+    const bool ok = query_interp_at(cfg, corner, pe, v);
+    if (e == 0) {
+      if (ok) { flags |= kQueryInterpolated; dist = v; }
+      continue;
+    }
+    if (!ok) break;
+    if (e & 1) { dplus = v; continue; }
+    const float gv = (dplus - v) / (2.0f * vs);
+    if (a == 0) ga[0] = gv; else if (a == 1) ga[1] = gv; else ga[2] = gv;
+    if (e == 6) { flags |= kQueryGradient; gx = ga[0]; gy = ga[1]; gz = ga[2]; }
+  }
 }
 
 // need_interp / need_grad: evaluate D(p) / the gradient (for the flags or the outputs that carry them)
@@ -151,28 +193,9 @@ __global__ void __launch_bounds__(kQueryThreads) k_query_points(DevCfg cfg, MapR
             row = (const float*)(chunk + cfg.head_bytes) + (size_t)vox * cfg.C;
             flags = kQueryAllocated | (wgt > min_weight ? kQueryObserved : 0);
           }
-          // evaluation 0: D(p); 2a + 1 / 2a + 2: D(p + vs e_a) / D(p - vs e_a).  One loop (not unrolled): the probe code is emitted once.
-          const float vs = cfg.voxel_size;
-          float dplus = 0.0f, ga[3] = {0.0f, 0.0f, 0.0f};
-          const int e_first = (need_interp && (flags & kQueryObserved)) ? 0 : 1;   // the containing voxel is a corner of D(p)
-          const int e_end = need_grad ? 7 : 1;
-#pragma unroll 1
-          for (int e = e_first; e < e_end; ++e) {
-            const int a = (e - 1) >> 1;
-            const float off = (e & 1) ? vs : -vs;
-            const F3 pe = f3(a == 0 ? p.x + off : p.x, a == 1 ? p.y + off : p.y, a == 2 ? p.z + off : p.z);
-            float v;
-            const bool ok = query_interp(cfg, map, w, pe, min_weight, v);
-            if (e == 0) {
-              if (ok) { flags |= kQueryInterpolated; interp = v; }
-              continue;
-            }
-            if (!ok) break;
-            if (e & 1) { dplus = v; continue; }
-            const float gv = (dplus - v) / (2.0f * vs);
-            if (a == 0) ga[0] = gv; else if (a == 1) ga[1] = gv; else ga[2] = gv;
-            if (e == 6) { flags |= kQueryGradient; gx = ga[0]; gy = ga[1]; gz = ga[2]; }
-          }
+          // the containing voxel is a corner of D(p)
+          query_stencil(cfg, TsdfCorner{cfg, map, w, min_weight}, p, need_interp && (flags & kQueryObserved), need_grad, flags, interp,
+                        gx, gy, gz);
         }
       }
       if (out.flags) out.flags[i] = (uint8_t)flags;

@@ -41,7 +41,7 @@ def kernel_name(key):
     if "k_esdf_sites" in key:
         return "k_esdf_sites"
     for a in "012":
-        if f"k_esdf_pass<{a}>" in key or f"k_esdf_passILi{a}E" in key:
+        if f"k_esdf_pass<{a}" in key or f"k_esdf_passILi{a}E" in key:
             return f"k_esdf_pass<{a}>"
     return key
 
