@@ -11,6 +11,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <memory>
+#include <numeric>
 #include <string>
 #include <type_traits>
 #include <unordered_map>
@@ -606,6 +607,13 @@ int finish_frame(ksg_integrator* h, ksg_frame_stats* stats) {
   if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
   return KSG_OK;
 }
+// The prologue of a host-buffer entry, which sees the map only once every submitted frame has completed: the device idle, the pending
+// frames completed, and their status.
+int complete_frames(ksg_integrator* h) {
+  KSG_CUDA(cudaSetDevice(h->device));
+  KSG_CUDA(cudaDeviceSynchronize());
+  return finish_frame(h, nullptr);
+}
 
 // fast: ApproxHashSet resets (fast.cpp:165-170, A.4), once per frame before any point is looked at
 int advance_sets(ksg_integrator* h, cudaStream_t s) {
@@ -1015,6 +1023,61 @@ int ensure_input(ksg_integrator* h, size_t bytes) {
   if (bytes > h->d_in_bytes) KSG_CUDA(h->res.regrow(&h->d_in, &h->d_in_bytes, bytes));
   return KSG_OK;
 }
+
+// A device copy of `v` in `tmp`, enqueued on `s`.
+template <typename T> cudaError_t upload(Resources& tmp, const std::vector<T>& v, cudaStream_t s, T** d) {
+  const cudaError_t e = tmp.device(d, v.size());
+  return e != cudaSuccess ? e : cudaMemcpyAsync(*d, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice, s);
+}
+
+// The device side of a host-buffer entry's host arrays: one temporary allocation per call, one 256-byte aligned slice per array.  The
+// caller declares the slices, each with the device pointer it sets, then run() makes them, uploads the inputs, launches, copies every
+// output slice to its host array on the call's stream and synchronises once.
+class HostStaging {
+ public:
+  // a slice for the host output `host` (NULL: not wanted, no slice and *dev = NULL, unless the kernel needs the slice anyway)
+  template <typename T> void out(T** dev, T* host, size_t count, bool kernel_needs = false) {
+    *dev = nullptr;
+    if (host || kernel_needs) add(dev, host, nullptr, count);
+  }
+  // a slice holding a copy of the host input `host`
+  template <typename T> void in(const T** dev, const T* host, size_t count) { add(dev, nullptr, host, count); }
+  // launch() enqueues the work on `s` once the device pointers are set, and returns a status
+  template <typename F> int run(ksg_integrator* h, cudaStream_t s, F&& launch) {
+    size_t total = 0;
+    for (const Slice& sl : slices_) total += aligned(sl.bytes);
+    uint8_t* d = nullptr;
+    KSG_CUDA(tmp_.device(&d, total));
+    for (Slice& sl : slices_) {
+      sl.at = d;
+      sl.bind(sl.dev, d);
+      if (sl.in) KSG_CUDA(cudaMemcpyAsync(d, sl.in, sl.bytes, cudaMemcpyHostToDevice, s));
+      d += aligned(sl.bytes);
+    }
+    { const int rcl = launch(); if (rcl) return rcl; }
+    KSG_CUDA(cudaGetLastError());
+    for (const Slice& sl : slices_)
+      if (sl.host) KSG_CUDA(cudaMemcpyAsync(sl.host, sl.at, sl.bytes, cudaMemcpyDeviceToHost, s));
+    KSG_CUDA(cudaStreamSynchronize(s));
+    return KSG_OK;
+  }
+
+ private:
+  struct Slice {
+    void* dev;                             // the T* that bind() points at the slice
+    void (*bind)(void* dev, uint8_t* at);
+    void* host;                            // an output's host array
+    const void* in;                        // an input's host array
+    size_t bytes;
+    uint8_t* at = nullptr;
+  };
+  template <typename T> void add(T** dev, void* host, const void* in, size_t count) {
+    slices_.push_back(Slice{dev, [](void* p, uint8_t* at) { *static_cast<T**>(p) = reinterpret_cast<T*>(at); }, host, in, count * sizeof(T)});
+  }
+  static size_t aligned(size_t bytes) { return (bytes + 255) / 256 * 256; }
+  std::vector<Slice> slices_;
+  Resources tmp_;
+};
 
 }  // namespace
 
@@ -1607,9 +1670,7 @@ int64_t update_log_count(const ksg_integrator* h) {
 
 int32_t ksg_set_update_log(ksg_integrator* h, int64_t capacity_voxels) {
   if (!h || capacity_voxels < 0 || capacity_voxels > (1ll << 30)) return KSG_ERR_INVALID_ARGUMENT;
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   for (void* p : {(void*)h->d_log_head, (void*)h->d_log_prior, (void*)h->h_log_head, (void*)h->h_log_prior}) h->res.release(p);
   h->d_log_head = nullptr; h->d_log_prior = nullptr; h->h_log_head = nullptr; h->h_log_prior = nullptr; h->log_cap = 0;
   h->merged_log_count = 0;
@@ -1658,9 +1719,7 @@ int32_t ksg_evaluate_labels(ksg_integrator* h, const ksg_world_object* objects, 
                             float checker_margin, int64_t* evaluated, int64_t* correct, int64_t* observed) {
   if (!h || n_objects < 0 || (n_objects > 0 && !objects) || n_objects > 4096) return KSG_ERR_INVALID_ARGUMENT;
   static_assert(sizeof(ksg_world_object) == sizeof(WorldObject), "ksg_world_object layout");
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   unsigned long long res[3] = {0, 0, 0};
   if (h->num_blocks > 0 && n_objects > 0) {
     Resources tmp;
@@ -1735,15 +1794,20 @@ void put_block_index(int32_t* block_index, int64_t i, uint64_t key) {
   block_index[3 * i] = b.x; block_index[3 * i + 1] = b.y; block_index[3 * i + 2] = b.z;
 }
 
-// The pool slots of the map's blocks in (z, y, x) order (keys are packed as z:y:x, biased: numeric order = (z, y, x)), and,
-// where block_index is given, the blocks' indices in that order.
+// The indices of `keys` in (z, y, x) order of their blocks (keys are packed as z:y:x, biased: numeric order = (z, y, x)).
+std::vector<int> zyx_order(const std::vector<uint64_t>& keys) {
+  std::vector<int> order(keys.size());
+  std::iota(order.begin(), order.end(), 0);
+  std::sort(order.begin(), order.end(), [&](int a, int b) { return keys[a] < keys[b]; });
+  return order;
+}
+
+// The pool slots of the map's blocks in (z, y, x) order, and, where block_index is given, the blocks' indices in that order.
 int slots_zyx(ksg_integrator* h, std::vector<int>* order, int32_t* block_index) {
   const int64_t nb = h->num_blocks;
   std::vector<uint64_t> keys((size_t)nb);
   KSG_CUDA(cudaMemcpy(keys.data(), h->map.slot_key, sizeof(uint64_t) * nb, cudaMemcpyDeviceToHost));
-  order->resize((size_t)nb);
-  for (int64_t i = 0; i < nb; ++i) (*order)[i] = (int)i;
-  std::sort(order->begin(), order->end(), [&](int a, int b) { return keys[a] < keys[b]; });
+  *order = zyx_order(keys);
   if (block_index) for (int64_t i = 0; i < nb; ++i) put_block_index(block_index, i, keys[(*order)[i]]);
   return KSG_OK;
 }
@@ -1780,9 +1844,7 @@ struct BlockStaging {
 int32_t ksg_extract_mesh(ksg_integrator* h, float min_weight, int64_t vertex_capacity, float* vertices, uint8_t* rgba, uint8_t* labels,
                          int64_t block_capacity, int32_t* block_index, int64_t* block_first_vertex, int64_t* n_vertices, int64_t* n_blocks) {
   if (!h || vertex_capacity < 0 || block_capacity < 0) return KSG_ERR_INVALID_ARGUMENT;
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   const int64_t nb = h->num_blocks;
   if (n_blocks) *n_blocks = nb;
   if (n_vertices) *n_vertices = 0;
@@ -1813,34 +1875,44 @@ int32_t ksg_extract_mesh(ksg_integrator* h, float min_weight, int64_t vertex_cap
   if (block_first_vertex) for (int64_t i = 0; i <= nb && i <= block_capacity; ++i) block_first_vertex[i] = first[i];
   if (!vertices && !rgba && !labels) return KSG_OK;                 // counting call
   if (total > vertex_capacity) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh: vertex capacity too small (n_vertices holds the need)");
-  if (total > 0) {
-    float* d_vtx = nullptr; uint32_t* d_rgba = nullptr; uint8_t* d_label = nullptr;
-    KSG_CUDA(tmp.device(&d_vtx, 3 * (size_t)total));
-    KSG_CUDA(tmp.device(&d_rgba, (size_t)total));
-    KSG_CUDA(tmp.device(&d_label, (size_t)total));
-    KSG_CUDA(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * nb, cudaMemcpyHostToDevice, s));
-    MeshBuf mb{d_vtx, d_rgba, d_label};
+  if (total == 0) return KSG_OK;
+  KSG_CUDA(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * nb, cudaMemcpyHostToDevice, s));
+  HostStaging st;
+  MeshBuf mb{};
+  st.out(&mb.vtx, vertices, 3 * (size_t)total, true);   // the kernel writes all three
+  st.out(&mb.rgba, reinterpret_cast<uint32_t*>(rgba), (size_t)total, true);
+  st.out(&mb.label, labels, (size_t)total, true);
+  return st.run(h, s, [&] {
     ++h->n_launches;
     k_mesh_blocks<true><<<grid, kMeshThreads, 0, s>>>(h->dc, h->map, d_slots, (int)nb, min_weight, d_first, nullptr, mb);
-    if (vertices) KSG_CUDA(cudaMemcpyAsync(vertices, d_vtx, sizeof(float) * 3 * total, cudaMemcpyDeviceToHost, s));
-    if (rgba) KSG_CUDA(cudaMemcpyAsync(rgba, d_rgba, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost, s));
-    if (labels) KSG_CUDA(cudaMemcpyAsync(labels, d_label, (size_t)total, cudaMemcpyDeviceToHost, s));
-    KSG_CUDA(cudaStreamSynchronize(s));
-    KSG_CUDA(cudaGetLastError());
-  }
-  return KSG_OK;
+    return KSG_OK;
+  });
 }
 
 namespace {
+bool query_wanted(const ksg_query_out& o) {
+  return o.flags || o.tsdf_distance || o.tsdf_weight || o.tsdf_rgba || o.sem_label || o.sem_priors || o.sem_rgba || o.distance || o.gradient;
+}
 // *work = false: the call has nothing to compute (n = 0 or no output wanted) and launches nothing
 int query_args(ksg_integrator* h, int64_t n, const float* xyz, float min_weight, const ksg_query_out* o, bool* work) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
   if (!o || n < 0 || !(min_weight >= 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "query: NULL out, n < 0 or a NaN / negative min_weight");
   if (n > 0 && !xyz) return h->fail(KSG_ERR_INVALID_ARGUMENT, "query: NULL points");
   if (h->dc.shard_count > 1) return h->fail(KSG_ERR_INVALID_ARGUMENT, "query: a sharded integrator holds only its own tiles");
-  *work = n > 0 && (o->flags || o->tsdf_distance || o->tsdf_weight || o->tsdf_rgba || o->sem_label || o->sem_priors || o->sem_rgba ||
-                    o->distance || o->gradient);
+  *work = n > 0 && query_wanted(*o);
   return KSG_OK;
+}
+// the slices of the wanted host outputs `o` of a point query at n points; *d receives their device pointers
+void stage_query_out(HostStaging* st, const ksg_query_out& o, size_t n, size_t C, ksg_query_out* d) {
+  st->out(&d->flags, o.flags, n);
+  st->out(&d->tsdf_distance, o.tsdf_distance, n);
+  st->out(&d->tsdf_weight, o.tsdf_weight, n);
+  st->out(&d->tsdf_rgba, o.tsdf_rgba, 4 * n);
+  st->out(&d->sem_label, o.sem_label, n);
+  st->out(&d->sem_priors, o.sem_priors, n * C);
+  st->out(&d->sem_rgba, o.sem_rgba, 4 * n);
+  st->out(&d->distance, o.distance, n);
+  st->out(&d->gradient, o.gradient, 3 * n);
 }
 void launch_query(ksg_integrator* h, int64_t n, const float* d_xyz, float min_weight, const ksg_query_out& o, cudaStream_t s) {
   static_assert(sizeof(ksg_query_out) == sizeof(QueryOut), "ksg_query_out layout");
@@ -1855,33 +1927,15 @@ void launch_query(ksg_integrator* h, int64_t n, const float* d_xyz, float min_we
 int32_t ksg_query_points(ksg_integrator* h, int64_t n, const float* xyz_G, float min_weight, const ksg_query_out* out) {
   bool work = false;
   { const int rca = query_args(h, n, xyz_G, min_weight, out, &work); if (rca) return rca; }
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   if (!work) return KSG_OK;
-  const ksg_query_out& o = *out;
-  const size_t N = (size_t)n, C = (size_t)h->dc.C;
-  // one device buffer: points, then every wanted output
-  const size_t sizes[10] = {12 * N, o.flags ? N : 0, o.tsdf_distance ? 4 * N : 0, o.tsdf_weight ? 4 * N : 0, o.tsdf_rgba ? 4 * N : 0,
-                            o.sem_label ? N : 0, o.sem_priors ? 4 * N * C : 0, o.sem_rgba ? 4 * N : 0, o.distance ? 4 * N : 0,
-                            o.gradient ? 12 * N : 0};
-  size_t off[10], total = 0;
-  for (int k = 0; k < 10; ++k) { off[k] = total; total += (sizes[k] + 255) / 256 * 256; }
-  Resources tmp;
-  uint8_t* d = nullptr;
-  KSG_CUDA(tmp.device(&d, total));
-  auto at = [&](int k) -> void* { return sizes[k] ? (void*)(d + off[k]) : nullptr; };
-  ksg_query_out dq{(uint8_t*)at(1), (float*)at(2), (float*)at(3), (uint8_t*)at(4), (uint8_t*)at(5), (float*)at(6), (uint8_t*)at(7),
-                   (float*)at(8), (float*)at(9)};
-  void* host[10] = {nullptr, o.flags, o.tsdf_distance, o.tsdf_weight, o.tsdf_rgba, o.sem_label, o.sem_priors, o.sem_rgba, o.distance, o.gradient};
+  HostStaging st;
+  const float* d_xyz = nullptr;
+  ksg_query_out dq{};
+  st.in(&d_xyz, xyz_G, 3 * (size_t)n);
+  stage_query_out(&st, *out, (size_t)n, (size_t)h->dc.C, &dq);
   cudaStream_t s = h->own_stream;
-  KSG_CUDA(cudaMemcpyAsync(d, xyz_G, sizes[0], cudaMemcpyHostToDevice, s));
-  launch_query(h, n, (const float*)d, min_weight, dq, s);
-  KSG_CUDA(cudaGetLastError());
-  for (int k = 1; k < 10; ++k)
-    if (sizes[k]) KSG_CUDA(cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s));
-  KSG_CUDA(cudaStreamSynchronize(s));
-  return KSG_OK;
+  return st.run(h, s, [&] { launch_query(h, n, d_xyz, min_weight, dq, s); return KSG_OK; });
 }
 
 int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, float min_weight, const ksg_query_out* d_out,
@@ -1897,9 +1951,6 @@ int32_t ksg_query_points_device(ksg_integrator* h, int64_t n, const float* d_xyz
 }
 
 namespace {
-bool query_wanted(const ksg_query_out& o) {
-  return o.flags || o.tsdf_distance || o.tsdf_weight || o.tsdf_rgba || o.sem_label || o.sem_priors || o.sem_rgba || o.distance || o.gradient;
-}
 // the checks both render entries share; fills the kernel's camera
 int render_args(ksg_integrator* h, const float* T, const double* K, int32_t width, int32_t height, float min_depth, float max_depth,
                 float min_weight, const ksg_render_out* o, RenderCam* c) {
@@ -1947,34 +1998,18 @@ int32_t ksg_render_view(ksg_integrator* h, const float* T_G_C, const double* K, 
                         float max_depth, float min_weight, const ksg_render_out* out) {
   RenderCam c{};
   { const int rca = render_args(h, T_G_C, K, width, height, min_depth, max_depth, min_weight, out, &c); if (rca) return rca; }
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
-  const ksg_query_out& o = out->at_hit;
-  const bool at_hit = query_wanted(o);
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
+  const bool at_hit = query_wanted(out->at_hit);
   if (!out->depth && !out->points_G && !at_hit) return KSG_OK;
-  const size_t N = (size_t)width * (size_t)height, C = (size_t)h->dc.C;
-  // one device buffer: depth, points (also when only at_hit outputs are wanted: the query reads them), then every wanted query output
-  const size_t sizes[11] = {out->depth ? 4 * N : 0, (out->points_G || at_hit) ? 12 * N : 0, o.flags ? N : 0, o.tsdf_distance ? 4 * N : 0,
-                            o.tsdf_weight ? 4 * N : 0, o.tsdf_rgba ? 4 * N : 0, o.sem_label ? N : 0, o.sem_priors ? 4 * N * C : 0,
-                            o.sem_rgba ? 4 * N : 0, o.distance ? 4 * N : 0, o.gradient ? 12 * N : 0};
-  size_t off[11], total = 0;
-  for (int k = 0; k < 11; ++k) { off[k] = total; total += (sizes[k] + 255) / 256 * 256; }
-  Resources tmp;
-  uint8_t* d = nullptr;
-  KSG_CUDA(tmp.device(&d, total));
-  auto at = [&](int k) -> void* { return sizes[k] ? (void*)(d + off[k]) : nullptr; };
-  ksg_query_out dq{(uint8_t*)at(2), (float*)at(3), (float*)at(4), (uint8_t*)at(5), (uint8_t*)at(6), (float*)at(7), (uint8_t*)at(8),
-                   (float*)at(9), (float*)at(10)};
-  void* host[11] = {out->depth, out->points_G, o.flags, o.tsdf_distance, o.tsdf_weight, o.tsdf_rgba, o.sem_label, o.sem_priors, o.sem_rgba,
-                    o.distance, o.gradient};
+  const size_t N = (size_t)width * (size_t)height;
+  HostStaging st;
+  float *d_depth = nullptr, *d_points = nullptr;
+  ksg_query_out dq{};
+  st.out(&d_depth, out->depth, N);
+  st.out(&d_points, out->points_G, 3 * N, at_hit);   // the query at the hits reads the points
+  stage_query_out(&st, out->at_hit, N, (size_t)h->dc.C, &dq);
   cudaStream_t s = h->own_stream;
-  launch_render(h, c, (float*)at(0), (float*)at(1), dq, s);
-  KSG_CUDA(cudaGetLastError());
-  for (int k = 0; k < 11; ++k)
-    if (host[k]) KSG_CUDA(cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s));
-  KSG_CUDA(cudaStreamSynchronize(s));
-  return KSG_OK;
+  return st.run(h, s, [&] { launch_render(h, c, d_depth, d_points, dq, s); return KSG_OK; });
 }
 
 int32_t ksg_render_view_device(ksg_integrator* h, const float* T_G_C_host, const double* K_host, int32_t width, int32_t height,
@@ -2076,15 +2111,61 @@ int esdf_args(ksg_integrator* h, float min_weight, float max_distance, int* W) {
   *W = (int)Wd;
   return KSG_OK;
 }
+
+// The sites step of ksg_compute_esdf and ksg_update_esdf: k_esdf_sites over the blocks at pool slots `slots`, whose site bytes go to
+// `site` in row = the slot (slot_rows, the device layer) or the position in `slots` (the batch entry).  *d_slots: the uploaded list (in
+// `tmp`); *has: each block's has-site byte, then, with `changed`, each block's changed byte.
+int esdf_sites(ksg_integrator* h, Resources& tmp, const std::vector<int>& slots, float min_weight, int slot_rows, uint8_t* site, bool changed,
+               int** d_slots, std::vector<uint8_t>* has) {
+  const int64_t n = (int64_t)slots.size(), n_out = changed ? 2 * n : n;
+  cudaStream_t s = h->own_stream;
+  uint8_t* d_has = nullptr;
+  KSG_CUDA(upload(tmp, slots, s, d_slots));
+  KSG_CUDA(tmp.device(&d_has, n_out));
+  ++h->n_launches;
+  k_esdf_sites<<<(int)std::min<int64_t>(n, (int64_t)h->sm_count * 8), kEsdfThreads, 0, s>>>(h->dc, h->map, *d_slots, (int)n, min_weight,
+                                                                                             slot_rows, site, d_has, changed ? d_has + n : nullptr);
+  has->resize((size_t)n_out);
+  KSG_CUDA(cudaMemcpyAsync(has->data(), d_has, n_out, cudaMemcpyDeviceToHost, s));
+  KSG_CUDA(cudaStreamSynchronize(s));
+  KSG_CUDA(cudaGetLastError());
+  return KSG_OK;
+}
+
+// The passes step of both entries: the three windowed passes, enqueued.  blocks[i] is the block of site row i of `site`, has[i] whether
+// it holds a site; the z work set is z_rows (row indices; NULL: every row, in row order), and eo.slots lists its pool slots on the
+// device.  The z pass writes eo in work set order or, with slot_rows, in the rows of the pool slots.  *st (NULL: not wanted) receives
+// the sizes of the three work sets.
+int esdf_passes(ksg_integrator* h, Resources& tmp, int W, int Rb, const std::vector<I3>& blocks, const std::vector<uint8_t>& has,
+                const std::vector<int>* z_rows, const uint8_t* site, const EsdfOut& eo, bool slot_rows, ksg_esdf_stats* st) {
+  const size_t V = (size_t)h->dc.vps * h->dc.vps * h->dc.vps;
+  const int64_t nz = z_rows ? (int64_t)z_rows->size() : (int64_t)blocks.size();
+  cudaStream_t s = h->own_stream;
+  EsdfWork wk;
+  wk.build(blocks, has, Rb, z_rows);
+  int *d_tx = nullptr, *d_ty = nullptr, *d_tz = nullptr, *d_a = nullptr, *d_b = nullptr;
+  KSG_CUDA(upload(tmp, wk.tx, s, &d_tx));
+  KSG_CUDA(upload(tmp, wk.ty, s, &d_ty));
+  KSG_CUDA(upload(tmp, wk.tz, s, &d_tz));
+  KSG_CUDA(tmp.device(&d_a, wk.n_x * V));
+  KSG_CUDA(tmp.device(&d_b, wk.n_y * V));
+  const EsdfOut none{nullptr, nullptr, nullptr, 0.0f, 0.0f};
+  h->n_launches += 3;
+  k_esdf_pass<0><<<esdf_grid(h, wk.n_x), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_x, W, Rb, d_tx, site, nullptr, d_a, nullptr, none);
+  k_esdf_pass<1><<<esdf_grid(h, wk.n_y), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_y, W, Rb, d_ty, nullptr, d_a, d_b, nullptr, none);
+  auto* const z_pass = slot_rows ? k_esdf_pass<2, true> : k_esdf_pass<2>;
+  z_pass<<<esdf_grid(h, nz), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)nz, W, Rb, d_tz, nullptr, d_b, nullptr, site, eo);
+  KSG_CUDA(cudaGetLastError());
+  if (st) { st->x_blocks = wk.n_x; st->y_blocks = wk.n_y; st->z_blocks = nz; }
+  return KSG_OK;
+}
 }  // namespace
 
 int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance, int64_t capacity_blocks, int32_t* block_index,
                          float* distance, uint8_t* flags) {
   int W = 0;
   { const int rca = esdf_args(h, min_weight, max_distance, &W); if (rca) return rca; }
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   const int64_t nb = h->num_blocks;
   if (nb > capacity_blocks) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf: block capacity too small");
   if (nb == 0) return KSG_OK;
@@ -2095,55 +2176,27 @@ int32_t ksg_compute_esdf(ksg_integrator* h, float min_weight, float max_distance
   if (!distance && !flags) return KSG_OK;
   const int vps = h->dc.vps, Rb = (W + vps - 1) / vps;
   const size_t V = (size_t)vps * vps * vps;
-  Resources tmp;
-  int* d_slots = nullptr; uint8_t* d_site = nullptr; uint8_t* d_has = nullptr;
-  KSG_CUDA(tmp.device(&d_slots, nb));
-  KSG_CUDA(tmp.device(&d_site, nb * V));
-  KSG_CUDA(tmp.device(&d_has, nb));
   cudaStream_t s = h->own_stream;
-  KSG_CUDA(cudaMemcpyAsync(d_slots, order.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s));
-  ++h->n_launches;
-  k_esdf_sites<<<(int)std::min<int64_t>(nb, (int64_t)h->sm_count * 8), kEsdfThreads, 0, s>>>(h->dc, h->map, d_slots, (int)nb, min_weight,
-                                                                                              0, d_site, d_has, nullptr);
-  std::vector<uint8_t> has((size_t)nb);
-  KSG_CUDA(cudaMemcpyAsync(has.data(), d_has, nb, cudaMemcpyDeviceToHost, s));
-  KSG_CUDA(cudaStreamSynchronize(s));
-  KSG_CUDA(cudaGetLastError());
-  std::vector<I3> alloc((size_t)nb);
-  for (int64_t i = 0; i < nb; ++i) alloc[i] = I3{index[3 * i], index[3 * i + 1], index[3 * i + 2]};
-  EsdfWork wk;
-  wk.build(alloc, has, Rb);
-  int *d_tx = nullptr, *d_ty = nullptr, *d_tz = nullptr, *d_a = nullptr, *d_b = nullptr;
-  float* d_dist = nullptr; uint8_t* d_flags = nullptr;
-  KSG_CUDA(tmp.device(&d_tx, wk.tx.size()));
-  KSG_CUDA(tmp.device(&d_ty, wk.ty.size()));
-  KSG_CUDA(tmp.device(&d_tz, wk.tz.size()));
-  KSG_CUDA(tmp.device(&d_a, wk.n_x * V));
-  KSG_CUDA(tmp.device(&d_b, wk.n_y * V));
-  if (distance) KSG_CUDA(tmp.device(&d_dist, nb * V));
-  if (flags) KSG_CUDA(tmp.device(&d_flags, nb * V));
-  KSG_CUDA(cudaMemcpyAsync(d_tx, wk.tx.data(), sizeof(int) * wk.tx.size(), cudaMemcpyHostToDevice, s));
-  KSG_CUDA(cudaMemcpyAsync(d_ty, wk.ty.data(), sizeof(int) * wk.ty.size(), cudaMemcpyHostToDevice, s));
-  KSG_CUDA(cudaMemcpyAsync(d_tz, wk.tz.data(), sizeof(int) * wk.tz.size(), cudaMemcpyHostToDevice, s));
-  const EsdfOut none{nullptr, nullptr, nullptr, 0.0f, 0.0f};
-  const EsdfOut eo{d_dist, d_flags, d_slots, min_weight, max_distance};
-  h->n_launches += 3;
-  k_esdf_pass<0><<<esdf_grid(h, wk.n_x), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_x, W, Rb, d_tx, d_site, nullptr, d_a, nullptr, none);
-  k_esdf_pass<1><<<esdf_grid(h, wk.n_y), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_y, W, Rb, d_ty, nullptr, d_a, d_b, nullptr, none);
-  k_esdf_pass<2><<<esdf_grid(h, nb), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)nb, W, Rb, d_tz, nullptr, d_b, nullptr, d_site, eo);
-  KSG_CUDA(cudaGetLastError());
-  if (distance) KSG_CUDA(cudaMemcpyAsync(distance, d_dist, sizeof(float) * nb * V, cudaMemcpyDeviceToHost, s));
-  if (flags) KSG_CUDA(cudaMemcpyAsync(flags, d_flags, nb * V, cudaMemcpyDeviceToHost, s));
-  KSG_CUDA(cudaStreamSynchronize(s));
-  return KSG_OK;
+  // site rows of its own, in (z, y, x) position order: the device layer is not touched
+  Resources tmp;
+  uint8_t* d_site = nullptr;
+  int* d_slots = nullptr;
+  std::vector<uint8_t> has;
+  KSG_CUDA(tmp.device(&d_site, nb * V));
+  { const int rcs = esdf_sites(h, tmp, order, min_weight, 0, d_site, false, &d_slots, &has); if (rcs) return rcs; }
+  std::vector<I3> blocks((size_t)nb);
+  for (int64_t i = 0; i < nb; ++i) blocks[i] = I3{index[3 * i], index[3 * i + 1], index[3 * i + 2]};
+  HostStaging st;
+  EsdfOut eo{nullptr, nullptr, d_slots, min_weight, max_distance};
+  st.out(&eo.distance, distance, nb * V);
+  st.out(&eo.flags, flags, nb * V);
+  return st.run(h, s, [&] { return esdf_passes(h, tmp, W, Rb, blocks, has, nullptr, d_site, eo, false, nullptr); });
 }
 
 int32_t ksg_update_esdf(ksg_integrator* h, float min_weight, float max_distance, ksg_esdf_stats* stats) {
   int W = 0;
   { const int rca = esdf_args(h, min_weight, max_distance, &W); if (rca) return rca; }
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   const int vps = h->dc.vps, Rb = (W + vps - 1) / vps;
   const size_t V = (size_t)vps * vps * vps;
   const int64_t nb = h->num_blocks;
@@ -2202,19 +2255,11 @@ int32_t ksg_update_esdf(ksg_integrator* h, float min_weight, float max_distance,
   if (!r_slots.empty()) {
     const int64_t nr = (int64_t)r_slots.size();
     Resources tmp;
-    int* d_r = nullptr; uint8_t* d_has = nullptr;
-    KSG_CUDA(tmp.device(&d_r, nr));
-    KSG_CUDA(tmp.device(&d_has, 2 * nr));   // has_site, then changed
     // rows new to the layer held no site before
     if (nb > prev) KSG_CUDA(cudaMemsetAsync(h->esdf_site + (size_t)prev * V, 0, (size_t)(nb - prev) * V, s));
-    KSG_CUDA(cudaMemcpyAsync(d_r, r_slots.data(), sizeof(int) * nr, cudaMemcpyHostToDevice, s));
-    ++h->n_launches;
-    k_esdf_sites<<<(int)std::min<int64_t>(nr, (int64_t)h->sm_count * 8), kEsdfThreads, 0, s>>>(h->dc, h->map, d_r, (int)nr, min_weight, 1,
-                                                                                                h->esdf_site, d_has, d_has + nr);
-    std::vector<uint8_t> has((size_t)(2 * nr));
-    KSG_CUDA(cudaMemcpyAsync(has.data(), d_has, 2 * nr, cudaMemcpyDeviceToHost, s));
-    KSG_CUDA(cudaStreamSynchronize(s));
-    KSG_CUDA(cudaGetLastError());
+    int* d_r = nullptr;
+    std::vector<uint8_t> has;   // has_site, then changed
+    { const int rcs = esdf_sites(h, tmp, r_slots, min_weight, 1, h->esdf_site, true, &d_r, &has); if (rcs) return rcs; }
     // S: the recomputed blocks whose site bytes changed; D = C + the allocated blocks within Rb (Chebyshev) of S, by a separable dilation
     // clamped to the allocated blocks' bounding box (an intermediate key takes the x, then the y coordinate of the allocated block it
     // reaches, so nothing outside the box is needed): the sets stay within |S| (2Rb + 1)^2 and the box, whatever the window
@@ -2246,32 +2291,12 @@ int32_t ksg_update_esdf(ksg_integrator* h, float min_weight, float max_distance,
     }
     std::sort(d_list.begin(), d_list.end(), [&](int a, int b) { return keys[a] < keys[b]; });
     // the passes over D, reading the stored site bytes of the whole map
-    std::vector<I3> alloc((size_t)nb);
-    for (int64_t i = 0; i < nb; ++i) alloc[i] = unpack_key(keys[i]);
-    EsdfWork wk;
-    wk.build(alloc, h->esdf_has_site, Rb, &d_list);
-    const int64_t nd = (int64_t)d_list.size();
-    st.x_blocks = wk.n_x;
-    st.y_blocks = wk.n_y;
-    st.z_blocks = nd;
-    int *d_tx = nullptr, *d_ty = nullptr, *d_tz = nullptr, *d_a = nullptr, *d_b = nullptr, *d_d = nullptr;
-    KSG_CUDA(tmp.device(&d_tx, wk.tx.size()));
-    KSG_CUDA(tmp.device(&d_ty, wk.ty.size()));
-    KSG_CUDA(tmp.device(&d_tz, wk.tz.size()));
-    KSG_CUDA(tmp.device(&d_a, wk.n_x * V));
-    KSG_CUDA(tmp.device(&d_b, wk.n_y * V));
-    KSG_CUDA(tmp.device(&d_d, nd));
-    KSG_CUDA(cudaMemcpyAsync(d_tx, wk.tx.data(), sizeof(int) * wk.tx.size(), cudaMemcpyHostToDevice, s));
-    KSG_CUDA(cudaMemcpyAsync(d_ty, wk.ty.data(), sizeof(int) * wk.ty.size(), cudaMemcpyHostToDevice, s));
-    KSG_CUDA(cudaMemcpyAsync(d_tz, wk.tz.data(), sizeof(int) * wk.tz.size(), cudaMemcpyHostToDevice, s));
-    KSG_CUDA(cudaMemcpyAsync(d_d, d_list.data(), sizeof(int) * nd, cudaMemcpyHostToDevice, s));
-    const EsdfOut none{nullptr, nullptr, nullptr, 0.0f, 0.0f};
+    std::vector<I3> blocks((size_t)nb);
+    for (int64_t i = 0; i < nb; ++i) blocks[i] = unpack_key(keys[i]);
+    int* d_d = nullptr;
+    KSG_CUDA(upload(tmp, d_list, s, &d_d));
     const EsdfOut eo{h->esdf_dist, h->esdf_flags, d_d, min_weight, max_distance};
-    h->n_launches += 3;
-    k_esdf_pass<0><<<esdf_grid(h, wk.n_x), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_x, W, Rb, d_tx, h->esdf_site, nullptr, d_a, nullptr, none);
-    k_esdf_pass<1><<<esdf_grid(h, wk.n_y), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)wk.n_y, W, Rb, d_ty, nullptr, d_a, d_b, nullptr, none);
-    k_esdf_pass<2, true><<<esdf_grid(h, nd), kEsdfThreads, 0, s>>>(h->dc, h->map, (int)nd, W, Rb, d_tz, nullptr, d_b, nullptr, h->esdf_site, eo);
-    KSG_CUDA(cudaGetLastError());
+    { const int rcp = esdf_passes(h, tmp, W, Rb, blocks, h->esdf_has_site, &d_list, h->esdf_site, eo, true, &st); if (rcp) return rcp; }
     KSG_CUDA(cudaStreamSynchronize(s));
   }
   h->esdf_full = false;
@@ -2290,12 +2315,7 @@ int32_t ksg_export_esdf(ksg_integrator* h, int32_t changed_only, int64_t capacit
                         float* distance, uint8_t* flags) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
   if (!h->esdf_valid) return h->fail(KSG_ERR_INVALID_ARGUMENT, "esdf export: no ksg_update_esdf since the handle was created, cleared or reset");
-  std::vector<int> all;
-  if (!changed_only) {
-    all.resize((size_t)h->esdf_blocks);
-    for (int64_t i = 0; i < h->esdf_blocks; ++i) all[i] = (int)i;
-    std::sort(all.begin(), all.end(), [&](int a, int b) { return h->esdf_keys[a] < h->esdf_keys[b]; });
-  }
+  const std::vector<int> all = changed_only ? std::vector<int>() : zyx_order(h->esdf_keys);
   const std::vector<int>& list = changed_only ? h->esdf_rewritten : all;
   const int64_t n = (int64_t)list.size();
   if (n_blocks) *n_blocks = n;
@@ -2305,20 +2325,17 @@ int32_t ksg_export_esdf(ksg_integrator* h, int32_t changed_only, int64_t capacit
   if ((!distance && !flags) || n == 0) return KSG_OK;
   KSG_CUDA(cudaSetDevice(h->device));
   const size_t V = (size_t)h->dc.vps * h->dc.vps * h->dc.vps;
-  Resources tmp;
-  int* d_slots = nullptr; float* d_dist = nullptr; uint8_t* d_flags = nullptr;
-  KSG_CUDA(tmp.device(&d_slots, n));
-  if (distance) KSG_CUDA(tmp.device(&d_dist, n * V));
-  if (flags) KSG_CUDA(tmp.device(&d_flags, n * V));
+  HostStaging st;
+  const int* d_slots = nullptr; float* d_dist = nullptr; uint8_t* d_flags = nullptr;
+  st.in(&d_slots, list.data(), (size_t)n);
+  st.out(&d_dist, distance, n * V);
+  st.out(&d_flags, flags, n * V);
   cudaStream_t s = h->own_stream;
-  KSG_CUDA(cudaMemcpyAsync(d_slots, list.data(), sizeof(int) * n, cudaMemcpyHostToDevice, s));
-  ++h->n_launches;
-  k_esdf_gather<<<esdf_grid(h, n), kEsdfThreads, 0, s>>>((int)V, d_slots, (int)n, h->esdf_dist, h->esdf_flags, d_dist, d_flags);
-  KSG_CUDA(cudaGetLastError());
-  if (distance) KSG_CUDA(cudaMemcpyAsync(distance, d_dist, sizeof(float) * n * V, cudaMemcpyDeviceToHost, s));
-  if (flags) KSG_CUDA(cudaMemcpyAsync(flags, d_flags, n * V, cudaMemcpyDeviceToHost, s));
-  KSG_CUDA(cudaStreamSynchronize(s));
-  return KSG_OK;
+  return st.run(h, s, [&] {
+    ++h->n_launches;
+    k_esdf_gather<<<esdf_grid(h, n), kEsdfThreads, 0, s>>>((int)V, d_slots, (int)n, h->esdf_dist, h->esdf_flags, d_dist, d_flags);
+    return KSG_OK;
+  });
 }
 
 namespace {
@@ -2346,31 +2363,20 @@ void launch_esdf_query(ksg_integrator* h, int64_t n, const float* d_xyz, const k
 int32_t ksg_query_esdf(ksg_integrator* h, int64_t n, const float* xyz_G, const ksg_esdf_query_out* out) {
   bool work = false;
   { const int rca = esdf_query_args(h, n, xyz_G, out, &work); if (rca) return rca; }
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   if (!work) return KSG_OK;
-  const ksg_esdf_query_out& o = *out;
   const size_t N = (size_t)n;
-  // one device buffer: points, then every wanted output
-  const size_t sizes[6] = {12 * N, o.flags ? N : 0, o.voxel_flags ? N : 0, o.voxel_distance ? 4 * N : 0, o.distance ? 4 * N : 0,
-                           o.gradient ? 12 * N : 0};
-  size_t off[6], total = 0;
-  for (int k = 0; k < 6; ++k) { off[k] = total; total += (sizes[k] + 255) / 256 * 256; }
-  Resources tmp;
-  uint8_t* d = nullptr;
-  KSG_CUDA(tmp.device(&d, total));
-  auto at = [&](int k) -> void* { return sizes[k] ? (void*)(d + off[k]) : nullptr; };
-  const ksg_esdf_query_out dq{(uint8_t*)at(1), (uint8_t*)at(2), (float*)at(3), (float*)at(4), (float*)at(5)};
-  void* host[6] = {nullptr, o.flags, o.voxel_flags, o.voxel_distance, o.distance, o.gradient};
+  HostStaging st;
+  const float* d_xyz = nullptr;
+  ksg_esdf_query_out dq{};
+  st.in(&d_xyz, xyz_G, 3 * N);
+  st.out(&dq.flags, out->flags, N);
+  st.out(&dq.voxel_flags, out->voxel_flags, N);
+  st.out(&dq.voxel_distance, out->voxel_distance, N);
+  st.out(&dq.distance, out->distance, N);
+  st.out(&dq.gradient, out->gradient, 3 * N);
   cudaStream_t s = h->own_stream;
-  KSG_CUDA(cudaMemcpyAsync(d, xyz_G, sizes[0], cudaMemcpyHostToDevice, s));
-  launch_esdf_query(h, n, (const float*)d, dq, s);
-  KSG_CUDA(cudaGetLastError());
-  for (int k = 1; k < 6; ++k)
-    if (sizes[k]) KSG_CUDA(cudaMemcpyAsync(host[k], at(k), sizes[k], cudaMemcpyDeviceToHost, s));
-  KSG_CUDA(cudaStreamSynchronize(s));
-  return KSG_OK;
+  return st.run(h, s, [&] { launch_esdf_query(h, n, d_xyz, dq, s); return KSG_OK; });
 }
 
 int32_t ksg_query_esdf_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, const ksg_esdf_query_out* d_out, void* cuda_stream) {
@@ -2386,9 +2392,7 @@ int32_t ksg_query_esdf_device(ksg_integrator* h, int64_t n, const float* d_xyz_G
 
 int32_t ksg_sync(ksg_integrator* h) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
   return KSG_OK;
 }
@@ -2487,9 +2491,7 @@ int32_t ksg_import_blocks(ksg_integrator* h, int64_t n, const int32_t* block_ind
   if (!h || n < 0 || (n > 0 && !block_index)) return KSG_ERR_INVALID_ARGUMENT;
   if (h->deferred_status) return h->fail(h->deferred_status, err_text(h->deferred_status));
   if (n == 0) return KSG_OK;
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   h->esdf_full = true;     // the import writes blocks without stamping them
   const DevCfg& dc = h->dc;
   HostBlockTable table;
@@ -2539,9 +2541,7 @@ int32_t ksg_import_blocks(ksg_integrator* h, int64_t n, const int32_t* block_ind
 
 int32_t ksg_device_map_view(ksg_integrator* h, int64_t* n_blocks, int64_t* block_stride_bytes, void** d_pool, void** d_block_keys) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   if (n_blocks) *n_blocks = h->num_blocks;
   if (block_stride_bytes) *block_stride_bytes = (int64_t)h->dc.block_stride;
   if (d_pool) *d_pool = h->map.pool;
@@ -2829,9 +2829,7 @@ int64_t ksg_debug_fast_timeline(ksg_integrator* h, int64_t* out64, int64_t* swee
 
 int32_t ksg_clear_map(ksg_integrator* h) {
   if (!h) return KSG_ERR_INVALID_ARGUMENT;
-  KSG_CUDA(cudaSetDevice(h->device));
-  KSG_CUDA(cudaDeviceSynchronize());
-  { const int rcp = finish_frame(h, nullptr); if (rcp) return rcp; }
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
   cudaStream_t s = h->own_stream;
   KSG_CUDA(cudaMemsetAsync(h->map.ht_keys, 0xFF, sizeof(uint64_t) * h->ht_cap, s));
   KSG_CUDA(cudaMemsetAsync(h->map.ht_slot, 0xFF, sizeof(int) * h->ht_cap, s));

@@ -152,7 +152,15 @@ def test_no_change_no_launch_and_device_frames_without_a_host_sync():
             gpu.integrate_depth_device(Tf, dd.data_ptr(), dl.data_ptr(), W, H, cam.K, stream=st.cuda_stream)
     s = gpu.update_esdf(1.0)
     assert s["full"] == 0 and s["changed_blocks"] > 0
-    _same(gpu.export_esdf(), gpu.esdf(1.0))
+    before = gpu.export_esdf()
+    _same(before, gpu.esdf(1.0))
+    # the batch entry at other parameters reads and writes none of the layer's state: the next update has nothing to do
+    gpu.esdf(0.6, min_weight=0.5)
+    gpu.set_profiling(False)
+    s = gpu.update_esdf(1.0)
+    assert s["full"] == 0 and s["changed_blocks"] == 0 and gpu.get_profile()["kernel_launches"] == 0
+    after = gpu.export_esdf()
+    assert after.keys() == before.keys() and all(after[k].tobytes() == before[k].tobytes() for k in before)
     gpu.close()
 
 
@@ -214,25 +222,29 @@ def test_queries_equal_the_twin_on_the_exported_layer(itype):
     got = gpu.query_esdf(np.concatenate([pts, inside]))
     _same({k: v[: len(pts)] for k, v in got.items()}, want)
     assert (got["flags"][len(pts):] == 0).all() and np.isnan(got["voxel_distance"][len(pts):]).all()
-    # unwanted outputs are never written; the device entry, in stream order
+    # unwanted outputs are never written; the device entry, in stream order, and the host entry with the same subset of outputs
     n = len(pts)
     guard = 0xA5
     dp = torch.from_numpy(pts).cuda()
     sizes = {"flags": n, "voxel_flags": n, "voxel_distance": 4 * n, "distance": 4 * n, "gradient": 12 * n}
     for keep in (("flags",), ("voxel_distance", "gradient"), ESDF_QUERY_FIELDS):
         bufs = {k: torch.full((sizes[k],), guard, dtype=torch.uint8, device="cuda") for k in ESDF_QUERY_FIELDS}
+        host = {k: np.full(sizes[k], guard, np.uint8) for k in ESDF_QUERY_FIELDS}
         st = torch.cuda.Stream()
         st.wait_stream(torch.cuda.current_stream())
         gpu.query_esdf_device(dp.data_ptr(), n, {k: bufs[k].data_ptr() for k in keep}, stream=st.cuda_stream)
         st.synchronize()
-        for k in ESDF_QUERY_FIELDS:
-            raw = bufs[k].cpu().numpy()
-            if k not in keep:
-                assert (raw == guard).all(), k
-                continue
-            dt = np.float32 if k in ("voxel_distance", "distance", "gradient") else np.uint8
-            v = raw.view(dt).reshape(want[k].shape)
-            _same({k: v}, {k: want[k]})
+        q = KsgEsdfQueryOut(**{k: host[k].ctypes.data for k in keep})
+        assert gpu.lib.ksg_query_esdf(gpu.handle, n, pts.ctypes.data, Ct.byref(q)) == 0
+        for raws in ({k: v.cpu().numpy() for k, v in bufs.items()}, host):
+            for k in ESDF_QUERY_FIELDS:
+                raw = raws[k]
+                if k not in keep:
+                    assert (raw == guard).all(), k
+                    continue
+                dt = np.float32 if k in ("voxel_distance", "distance", "gradient") else np.uint8
+                v = raw.view(dt).reshape(want[k].shape)
+                _same({k: v}, {k: want[k]})
     gpu.close()
 
 

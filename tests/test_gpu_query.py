@@ -160,16 +160,20 @@ def test_unrequested_outputs_are_never_written(wanted):
     n, C = len(p), cfg.num_labels
     guard = 0xA5
     out = _device_out(n, C, guard)
+    host = {k: v.cpu().numpy() for k, v in out.items()}                  # host arrays of the same shapes, every byte = guard
     d_p = torch.from_numpy(p).cuda()
     torch.cuda.synchronize()
     gpu.query_points_device(d_p.data_ptr(), n, {k: out[k].data_ptr() for k in wanted})
     gpu.sync()
+    # the host entry with the same subset of outputs
+    q = KsgQueryOut(**{k: host[k].ctypes.data for k in wanted})
+    assert gpu.lib.ksg_query_points(gpu.handle, n, p.ctypes.data, 1e-4, Ct.byref(q)) == 0
     want = qr.query(exp, cfg.voxel_size, cfg.voxels_per_side, p)
-    got = {k: v.cpu().numpy() for k, v in out.items()}
-    _same(got, want, wanted)
-    for k in QUERY_FIELDS:
-        if k not in wanted:
-            assert (got[k].view(np.uint8) == guard).all(), k
+    for got in ({k: v.cpu().numpy() for k, v in out.items()}, host):
+        _same(got, want, wanted)
+        for k in QUERY_FIELDS:
+            if k not in wanted:
+                assert (got[k].view(np.uint8) == guard).all(), k
     gpu.close()
 
 

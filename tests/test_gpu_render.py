@@ -11,7 +11,8 @@ import pytest
 import torch
 
 from kimera_semantics_b200 import synth
-from kimera_semantics_b200.capi import (RENDER_FIELDS, Integrator, KsgRenderOut, KSG_INTEGRATOR_FAST, KSG_INTEGRATOR_MERGED)
+from kimera_semantics_b200.capi import (QUERY_FIELDS, RENDER_FIELDS, Integrator, KsgError, KsgRenderOut, KSG_INTEGRATOR_FAST,
+                                        KSG_INTEGRATOR_MERGED)
 from parity_utils import frames, make_config
 from test_shim_cpu import demo, write_frames  # noqa: F401
 from test_gpu_more import read_shim_output
@@ -112,7 +113,7 @@ def test_device_render_is_ordered_behind_device_frames_without_a_host_sync(itype
     gpu.close()
 
 
-@pytest.mark.parametrize("wanted", [("depth",), ("points_G",), RENDER_FIELDS])
+@pytest.mark.parametrize("wanted", [("depth",), ("points_G",), ("sem_label", "gradient"), RENDER_FIELDS])
 def test_unrequested_outputs_are_never_written(wanted):
     C, vs = 21, 0.05
     cfg = make_config(KSG_INTEGRATOR_MERGED, vs, C, max_points=W * H, max_updates=16 << 20)
@@ -124,13 +125,22 @@ def test_unrequested_outputs_are_never_written(wanted):
     guard = 0xA5
     out = _device_out(W * H, C, guard)
     torch.cuda.synchronize()
-    gpu.render_device(T, _K(cam), W, H, 0.1, 6.0, {k: out[k].data_ptr() for k in wanted})
+    ptrs = {k: out[k].data_ptr() for k in wanted}
+    on_device = wanted
+    if "points_G" not in wanted and set(wanted) & set(QUERY_FIELDS):
+        # at_hit outputs without points_G: the device entry refuses them (its query reads points_G); the host entry stages the points
+        with pytest.raises(KsgError):
+            gpu.render_device(T, _K(cam), W, H, 0.1, 6.0, ptrs)
+        on_device = ()
+    else:
+        gpu.render_device(T, _K(cam), W, H, 0.1, 6.0, ptrs)
     gpu.sync()
     want = _flat(rr.render(exp, vs, cfg.voxels_per_side, T, _K(cam), W, H, 0.1, 6.0))
     got = {k: v.cpu().numpy() for k, v in out.items()}
-    _same(got, want, wanted)
+    if on_device:
+        _same(got, want, on_device)
     for k in RENDER_FIELDS:
-        if k not in wanted:
+        if k not in on_device:
             assert (got[k].view(np.uint8) == guard).all(), k
     # the host entry writes exactly what it is asked for, too
     host = gpu.render(T, _K(cam), W, H, 0.1, 6.0, fields=wanted)
