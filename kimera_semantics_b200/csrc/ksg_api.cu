@@ -218,11 +218,9 @@ struct ksg_integrator {
   uint32_t *iota = nullptr;
 
   // fast
-  int *start_next = nullptr, *start_min = nullptr, *start_max = nullptr;
+  StartRec* start_rec = nullptr;     // [2^20] empty between frames (StartBuf)
   uint32_t *start_table = nullptr;
-  int *s_base = nullptr, *s_visits = nullptr;   // start-set slots shared by several cells (FastFrame)
-  uint32_t *s_hmin = nullptr, *s_hmax = nullptr;
-  uint8_t *clear_ff = nullptr, *clear_00 = nullptr;   // per-frame cleared regions behind several of the arrays above (see ksg_create)
+  int* start_touched = nullptr;
   uint64_t set_offset = 0;  // both ApproxHashSets share reset times, hence one offset (fast.cpp:165-170)
   int64_t reset_counter = 0;
   int* cast_seq = nullptr;
@@ -287,7 +285,8 @@ struct ksg_integrator {
   // fast frame driver (ksg_fast.cuh): no host read-back inside the frame
   FastCounters* d_fc = nullptr;
   FastCounters* h_fc = nullptr;      // pinned
-  int *blk_cnt = nullptr, *blk_off = nullptr, *warp_cnt = nullptr, *warp_off = nullptr, *seq_of_i = nullptr;
+  int *blk_cnt = nullptr, *blk_off = nullptr, *warp_off = nullptr, *seq_of_i = nullptr;
+  uint32_t* cast_bits = nullptr;     // empty between frames (FastFrame)
   uint32_t* keys32 = nullptr;
   int *tile_cnt = nullptr, *tile_slot = nullptr;
   TileDesc* tile_list = nullptr;
@@ -402,6 +401,11 @@ int reset_map(ksg_integrator* h, cudaStream_t s) {
   if (h->start_table) KSG_CUDA(cudaMemsetAsync(h->start_table, 0xFF, sizeof(uint32_t) * kSetSize, s));
   if (h->o3.table) KSG_CUDA(cudaMemsetAsync(h->o3.table, 0xFF, sizeof(uint32_t) * kSetSize, s));
   if (h->d_fc) KSG_CUDA(cudaMemsetAsync(h->d_fc, 0, sizeof(FastCounters), s));
+  if (h->start_rec) {   // every consumer empties what it decided; a reset does not rely on it
+    KSG_CUDA(cudaMemset2DAsync(&h->start_rec->first, sizeof(StartRec), 0xFF, 2 * sizeof(uint32_t), kSetSize, s));   // first, hmin
+    KSG_CUDA(cudaMemset2DAsync(&h->start_rec->hmax, sizeof(StartRec), 0x00, 2 * sizeof(uint32_t), kSetSize, s));    // hmax, visits
+  }
+  if (h->cast_bits) KSG_CUDA(cudaMemsetAsync(h->cast_bits, 0, sizeof(uint32_t) * ((size_t)h->cap_points / 32 + 64), s));
   if (h->o3.stamp_max) {   // (sweep 0, nobody): max word 0, min word all ones
     KSG_CUDA(cudaMemsetAsync(h->o3.stamp_max, 0x00, sizeof(uint64_t) * kSetSize, s));
     KSG_CUDA(cudaMemsetAsync(h->o3.stamp_min, 0xFF, sizeof(uint64_t) * kSetSize, s));
@@ -621,7 +625,7 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   FastFrame f{};
   f.cfg = h->dc; f.T = T; f.in = fin; f.in.pix_list = nullptr; f.in.point_of_seq = nullptr;
   f.luts = h->d_luts; f.cnt = h->d_cnt; f.fc = h->d_fc; f.map = h->map;
-  f.sb = StartBuf{h->start_next, h->start_min, h->start_max, h->start_table};
+  f.sb = StartBuf{h->start_rec, h->start_table, h->start_touched, sorted ? h->point_of_seq : nullptr};
   f.set_offset = h->set_offset;
   f.capacity = cap;
   f.n_count_blocks = (cap + kCountBlock - 1) / kCountBlock;
@@ -630,9 +634,8 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   f.profile = (h->profiling && !h->profile_marks_only) ? 1 : 0;
   f.prof_marks = h->profiling ? 1 : 0;
   f.seq_of_i = sorted ? h->seq_of_i : nullptr;
-  f.block_cnt = h->blk_cnt; f.block_off = h->blk_off; f.warp_cnt = h->warp_cnt; f.warp_off = h->warp_off;
-  f.pt_pG = h->pt_pG; f.pt_label = h->pt_label; f.pt_flags = h->pt_flags; f.pt_color = h->pt_color; f.pt_key = h->pt_key;
-  f.cast_flag = h->flags8;
+  f.block_cnt = h->blk_cnt; f.block_off = h->blk_off; f.cast_bits = h->cast_bits; f.warp_off = h->warp_off;
+  f.pt_key = h->pt_key; f.pt_pix = h->pix_list;
   f.cast_seq = h->cast_seq; f.ray_param = h->ray_param; f.ray_label = h->ray_label; f.ray_flags = h->ray_flags; f.ray_color = h->ray_color;
   f.ray_state = h->ray_state; f.ext_off = h->ext_off;
   f.rec_cap = h->rec_cap; f.keys = h->keys32;
@@ -642,16 +645,14 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   f.wl_listed = h->wl;
   f.wl_list[0] = h->wl + h->cap_points; f.wl_list[1] = h->wl + 2 * (size_t)h->cap_points;
   f.log_head = h->d_log_head; f.log_prior = h->d_log_prior; f.log_cap = h->log_cap;
-  f.s_base = h->s_base; f.s_hmin = h->s_hmin; f.s_hmax = h->s_hmax; f.s_visits = h->s_visits;
   f.mixed_list = h->mixed_list; f.m_list = h->m_list;
 
   if (h->profiling) {
     cudaEventRecord(h->ev[0], s);
     KSG_CUDA(cudaMemsetAsync(h->d_fc->dbg, 0, sizeof(h->d_fc->dbg), s));
   }
-  KSG_CUDA(cudaMemsetAsync(h->clear_ff, 0xFF, (size_t)kSetSize * 16, s));
-  KSG_CUDA(cudaMemsetAsync(h->clear_00, 0x00, (size_t)kSetSize * 13, s));
-  KSG_CUDA(cudaMemsetAsync(h->start_min, 0x7F, sizeof(int) * kSetSize, s));
+  KSG_CUDA(cudaMemsetAsync(h->o3.head, 0xFF, sizeof(int) * kSetSize, s));
+  KSG_CUDA(cudaMemsetAsync(h->o3.slot_cnt, 0x00, sizeof(int) * kSetSize, s));
   const int B = 256;
   ++h->n_launches;
   if (in.d_depth) k_fast_count<<<f.n_count_blocks, 256, 0, s>>>(f);
@@ -670,7 +671,7 @@ int integrate_fast(ksg_integrator* h, const InputDesc& in, const FrameIn& fin, c
   if (in.d_depth) k_fast_classify<true><<<f.n_count_blocks, 256, 0, s>>>(f);
   else k_fast_classify<false><<<grid_for(cap, B), B, 0, s>>>(f);
   ++h->n_launches;
-  k_fast_start_eval3<<<(cap + kEvalBlock - 1) / kEvalBlock, kEvalBlock, 0, s>>>(f);
+  k_fast_start_slots<<<std::min(grid_for(cap, B), 4 * h->sm_count), B, 0, s>>>(f);
   if (h->profiling) cudaEventRecord(h->ev[1], s);
   {
     // The fixpoint is reached within rays + 1 sweeps, plus one that changes nothing (DESIGN.md section 4), and a frame casts at
@@ -1239,9 +1240,12 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
   const size_t N = (size_t)cfg->max_points;
   h->cap_points = cfg->max_points;
   const bool fast = cfg->integrator_type == KSG_INTEGRATOR_FAST;
-  KSG_CUDA(res.device(&h->pt_pC, N)); KSG_CUDA(res.device(&h->pt_pG, N));
-  KSG_CUDA(res.device(&h->pt_label, N)); KSG_CUDA(res.device(&h->pt_flags, N));
-  KSG_CUDA(res.device(&h->pt_color, N)); KSG_CUDA(res.device(&h->pt_key, N));
+  if (!fast) {   // merged's per-point state (fast keeps only the start-set key and the pixel per input index)
+    KSG_CUDA(res.device(&h->pt_pC, N)); KSG_CUDA(res.device(&h->pt_pG, N));
+    KSG_CUDA(res.device(&h->pt_label, N)); KSG_CUDA(res.device(&h->pt_flags, N));
+    KSG_CUDA(res.device(&h->pt_color, N));
+  }
+  KSG_CUDA(res.device(&h->pt_key, N));
   KSG_CUDA(res.device(&h->flags8, 2 * N));
   KSG_CUDA(res.device(&h->pix_list, N));
   KSG_CUDA(res.device(&h->iota, N));
@@ -1252,17 +1256,9 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
   KSG_CUDA(res.device(&h->ray_param, N)); KSG_CUDA(res.device(&h->ray_flags, N)); KSG_CUDA(res.device(&h->nsteps, N));
   long long rec_cap = cfg->max_updates > 0 ? cfg->max_updates : (fast ? std::max<long long>(4ll << 20, 64ll * (long long)N) : (64ll << 20));
   if (fast) {
-    KSG_CUDA(res.device(&h->start_next, N)); KSG_CUDA(res.device(&h->start_table, kSetSize));
-    // per-frame cleared arrays live in two contiguous regions, so that a frame needs three memsets instead of seven:
-    //   0xFF: [s_base | start_max | s_hmin | o3.head]               4 + 4 + 4 + 4 bytes per slot
-    //   0x00: [o3.slot_cnt | (unused) | s_hmax | s_visits]          4 + 1 + 4 + 4 bytes per slot
-    KSG_CUDA(res.device(&h->clear_ff, (size_t)kSetSize * 16));
-    KSG_CUDA(res.device(&h->clear_00, (size_t)kSetSize * 13));
-    h->s_base = (int*)h->clear_ff; h->start_max = h->s_base + kSetSize; h->s_hmin = (uint32_t*)(h->start_max + kSetSize);
-    h->o3.head = (int*)(h->clear_ff + (size_t)kSetSize * 12);
-    h->o3.slot_cnt = (int*)h->clear_00;
-    h->s_hmax = (uint32_t*)(h->clear_00 + (size_t)kSetSize * 5); h->s_visits = (int*)(h->clear_00 + (size_t)kSetSize * 9);
-    KSG_CUDA(res.device(&h->start_min, kSetSize));
+    KSG_CUDA(res.device(&h->start_rec, kSetSize)); KSG_CUDA(res.device(&h->start_table, kSetSize));
+    KSG_CUDA(res.device(&h->start_touched, N));
+    KSG_CUDA(res.device(&h->o3.head, kSetSize)); KSG_CUDA(res.device(&h->o3.slot_cnt, kSetSize));   // cleared per frame
     KSG_CUDA(res.device(&h->cast_seq, N));
     KSG_CUDA(res.device(&h->ray_label, N)); KSG_CUDA(res.device(&h->ray_color, N));
     KSG_CUDA(res.device(&h->ray_state, N)); KSG_CUDA(res.device(&h->ext_off, N * kExtSegs));
@@ -1402,7 +1398,7 @@ int32_t ksg_create(const ksg_config* cfg, ksg_integrator** out) {
     std::memset(h->h_fc_base, 0, 2 * sizeof(FastCounters));
     h->h_fc = h->h_fc_base;
     KSG_CUDA(res.device(&h->blk_cnt, N / kCountBlock + 2)); KSG_CUDA(res.device(&h->blk_off, N / kCountBlock + 2));
-    KSG_CUDA(res.device(&h->warp_cnt, N / 32 + 64)); KSG_CUDA(res.device(&h->warp_off, N / 32 + 64));
+    KSG_CUDA(res.device(&h->cast_bits, N / 32 + 64)); KSG_CUDA(res.device(&h->warp_off, N / 32 + 64));
     if (cfg->integration_order_mode == KSG_ORDER_SORTED) KSG_CUDA(res.device(&h->seq_of_i, N));
     KSG_CUDA(res.device(&h->keys32, (size_t)rec_cap));
     const size_t n_tk = (size_t)h->ht_cap * dc.tiles_per_block;

@@ -321,13 +321,17 @@ __device__ __forceinline__ void fast3_ray_setup(const FastFrame& f, int r, int n
   const long long t_begin = f.profile ? clock64() : 0;
   long long t_ins = 0;
   if (r < n_cast) {
+    // the cast point again from its input (fast_point, as k_fast_classify computed it)
     const int seq = f.cast_seq[r];
-    const float4 p = f.pt_pG[seq];
-    const uint8_t fl = f.pt_flags[seq];
+    const int i = f.sb.i_of_seq ? f.sb.i_of_seq[seq] : mixed_index(seq, __ldcg(&f.cnt->n_points));
+    const int pix = f.in.depth ? f.pt_pix[i] : i;
+    const FastPoint q = fast_point(f, pix, f.in.depth ? __ldg(f.in.depth + pix) : 0.0f);
+    const float4 p = make_float4(q.pG.x, q.pG.y, q.pG.z, q.w);
+    const uint8_t fl = (q.valid ? 1 : 0) | (q.clearing ? 2 : 0);
     f.ray_param[r] = p;
-    f.ray_label[r] = f.pt_label[seq];
+    f.ray_label[r] = q.label;
     f.ray_flags[r] = fl;
-    f.ray_color[r] = f.pt_color[seq];
+    f.ray_color[r] = q.color;
     if (f.profile) dbg_max(f, 12, clock64() - t_begin);
     Dda d;
     raycaster_init(d, f3(f.T.tx, f.T.ty, f.T.tz), f3(p.x, p.y, p.z), (fl & 2) != 0, cfg.carving != 0, cfg.max_ray, cfg.vsi, cfg.tp.trunc,
@@ -627,37 +631,47 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
   int tl = 0;
   timeline_mark(f, tl++);
   extern __shared__ int s_sort[];            // kSortPerWarp ints per warp
-  // ---- phase 0a: start-set slots shared by several cells: every visitor files itself in the slot's list
+  // ---- phase 0a: start-set slots shared by several cells: every visitor files its sequence position in the slot's list (the
+  // records of the other slots were emptied by k_fast_start_slots: no visits)
   const int n_mixed = ((volatile int*)&f.fc->n_mixed)[0];
   if (n_mixed > 0) {
     if (gtid0 == 0) f.fc->wl_claim[0] = 0;
-    for (int seq = gtid0; seq < n_points; seq += gthreads) {
-      const uint64_t v = f.pt_key[seq];
+    for (int i = gtid0; i < n_points; i += gthreads) {
+      const uint64_t v = __ldcg(&f.pt_key[i]);
       if (v == ~0ull) continue;
-      const uint32_t slot = (uint32_t)v & kSetMask;
-      if (f.s_hmin[slot] != f.s_hmax[slot]) f.m_list[f.s_base[slot] + f.sb.next[seq]] = seq;
+      StartRec* r = &f.sb.rec[(uint32_t)v & kSetMask];
+      if (__ldcg(&r->visits) != 0) f.m_list[atomicAdd(&r->first, 1u)] = f.seq_of_i ? f.seq_of_i[i] : inv_mixed_index(i, n_points);
     }
     solve_barrier(bar, epoch);
     timeline_mark(f, 57);
-    // ---- phase 0b: one warp per such slot: visitors in sequence order; a visitor is cast iff its predecessor carried another value.
+    // ---- phase 0b: one warp per such slot: visitors in sequence order; the first is cast iff the table holds another value, a later
+    // one iff its predecessor carried another value; the table takes the last visitor's value and the record is emptied.
     // Visitor counts vary by two or three orders of magnitude: a warp's first slot is its warp index, the next ones are claimed
     // from a cursor (wl_claim[0], zeroed in phase 0a; the sweeps zero it again before they use it), so no warp draws several
     // large slots while others idle.
     const int warps_total = gthreads >> 5;
     int* scratch = s_sort + (threadIdx.x >> 5) * kSortPerWarp;
+    auto key_of_seq = [&](int seq) { return __ldcg(&f.pt_key[f.sb.i_of_seq ? f.sb.i_of_seq[seq] : mixed_index(seq, n_points)]); };
     for (int mi = (threadIdx.x >> 5) * gridDim.x + blockIdx.x; mi < n_mixed;) {
       const int slot = f.mixed_list[mi];
-      const int n = __ldcg(&f.s_visits[slot]);
-      int* seg = f.m_list + __ldcg(&f.s_base[slot]);
+      StartRec* rec = &f.sb.rec[slot];
+      const int n = (int)__ldcg(&rec->visits);
+      int* seg = f.m_list + ((int)__ldcg(&rec->first) - n);   // phase 0a left the cursor at the end of the list
       int* a = seg;
       if (n <= kSortPerWarp) { for (int i = lane; i < n; i += 32) scratch[i] = __ldcg(&seg[i]); a = scratch; }
       __syncwarp();
       warp_sort_i32(a, n, lane);
-      for (int i = 1 + lane; i < n; i += 32) {
-        const int pa = a[i - 1], pb = a[i];
-        if (f.pt_key[pa] != f.pt_key[pb]) { f.cast_flag[pb] = 1; atomicAdd(&f.warp_cnt[pb >> 5], 1); }
+      for (int i = lane; i < n; i += 32) {
+        const int sb = a[i];
+        const uint64_t kb = key_of_seq(sb);
+        const bool cast = i == 0 ? f.sb.table[slot] != (uint32_t)(kb >> kSetBits) : key_of_seq(a[i - 1]) != kb;
+        if (cast) atomicOr(&f.cast_bits[sb >> 5], 1u << (sb & 31));
       }
       __syncwarp();
+      if (lane == 0) {
+        f.sb.table[slot] = (uint32_t)(key_of_seq(a[n - 1]) >> kSetBits);
+        *(uint4*)rec = start_rec_empty();
+      }
       if (f.profile && lane == 0) { dbg_max(f, 8, n); dbg_add(f, 9, n); }
       int next = 0;
       if (lane == 0) next = warps_total + atomicAdd(&f.fc->wl_claim[0], 1);
@@ -666,20 +680,21 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
     solve_barrier(bar, epoch);
     timeline_mark(f, 58);
   }
-  // ---- phase 0c: offsets of the cast points (block 0), then compaction in sequence order (= ray rank order)
+  // ---- phase 0c: offsets of the cast points (block 0), then compaction in sequence order (= ray rank order); every word of the
+  // cast bits is cleared once read
+  const int n_words = (f.capacity + 31) >> 5;
   if (blockIdx.x == 0) {
-    const int n_warps32 = (f.capacity + 31) >> 5;
-    const int total = block_scan_array(f.warp_cnt, f.warp_off, n_warps32);
+    const int total = block_scan_array<true>((const int*)f.cast_bits, f.warp_off, n_words);
     if (threadIdx.x == 0) cnt->n_cast = total;
   }
   solve_barrier(bar, epoch);
   timeline_mark(f, 59);
   const int n_cast = ((volatile int*)&cnt->n_cast)[0];
-  for (int base = (gtid0 & ~31); base < n_points; base += gthreads) {
-    const int seq = base + lane;
-    const bool c = seq < n_points && __ldcg(&f.cast_flag[seq]) != 0;
-    const unsigned m = __ballot_sync(0xffffffffu, c);
-    if (c) f.cast_seq[__ldcg(&f.warp_off[seq >> 5]) + __popc(m & ((1u << lane) - 1u))] = seq;
+  for (int w = gtid0; w < n_words; w += gthreads) {
+    uint32_t m = __ldcg(&f.cast_bits[w]);
+    if (m == 0u) continue;
+    f.cast_bits[w] = 0u;
+    for (int at = __ldcg(&f.warp_off[w]); m; m &= m - 1u) f.cast_seq[at++] = (w << 5) | (__ffs(m) - 1);
   }
   const int sweep_base0 = ((volatile int*)&f.fc->sweep_base)[0];   // sweep ids are monotonic across frames (31 bits: never wraps in practice)
   if (gtid0 == 0) for (int k = 0; k < 4; ++k) { f.fc->wl_claim[k] = 0; f.fc->wl_count[k] = 0; }
@@ -763,6 +778,7 @@ __global__ void __launch_bounds__(kSolveThreads, 1) k_fast_solve3(FastFrame f, i
     if (f.profile) { f.fc->dbg[10] = ((volatile int*)&f.fc->n_mixed)[0]; f.fc->dbg[11] = ((volatile int*)&cnt->n_cast)[0]; }
     f.fc->n_mixed = 0;
     f.fc->m_cursor = 0;
+    f.fc->n_touched = 0;
     f.fc->log_count = 0;
   }
   timeline_mark(f, tl++);
