@@ -450,6 +450,45 @@ typedef struct ksg_esdf_query_out {
 int32_t ksg_query_esdf(ksg_integrator* h, int64_t n, const float* xyz_G, const ksg_esdf_query_out* out);
 int32_t ksg_query_esdf_device(ksg_integrator* h, int64_t n, const float* d_xyz_G, const ksg_esdf_query_out* d_out, void* cuda_stream);
 
+/* The semantic mesh kept on the device and re-meshed only where a map change can reach it (what voxblox's TsdfServer::updateMesh does
+ * while the map grows).  The layer holds, per pool slot, the block's vertices as ksg_extract_mesh emits them, in one device arena laid
+ * out by slot; the first ksg_update_mesh allocates it and ksg_destroy frees it.  After every update the layer equals what
+ * ksg_extract_mesh(min_weight) returns for the map at that moment, bit for bit: same kernel (csrc/ksg_mesh.cuh states the dirty-set
+ * rule, why it is exact, and the coordinate bound it needs).
+ * ksg_update_mesh: rejects a NULL handle, a NaN or negative min_weight and a sharded integrator; completes the pending frame, updates
+ * the layer and returns when done.  The update is full (every block re-meshed) on the first call, after a change of min_weight, after
+ * any ksg_clear_map, ksg_reset or ksg_import_blocks since the last update, and after an update that found a block of the map beyond
+ * the coordinate bound (|block index| + 1) * voxels_per_side + 2 <= 2^18 (that update is exact: the block is new, so it is
+ * re-meshed), until a clear or reset.  Otherwise it re-meshes R: the blocks touched or allocated since the last
+ * update (C) and their allocated lower neighbours at the 7 offsets -e, e in {0,1}^3.  No stamp and no allocation since the last update:
+ * no launch.  Otherwise 1 kernel launch when R turns out empty, else 5; the host reads back a fixed number of scalars, nothing per
+ * block.  `stats` (may be NULL) receives the counts below.  A call that fails after its argument checks leaves the layer untrusted:
+ * export and view are refused and the next update is full.
+ * ksg_export_mesh: the layer as of the last update, in ksg_extract_mesh's layout and sizing convention (counting call with vertices =
+ * rgba = labels = NULL; KSG_ERR_INVALID_ARGUMENT when a capacity is too small, n_vertices / n_blocks still report the need).
+ * changed_only = 0: every block the layer covers, in (z, y, x) order - equal to ksg_extract_mesh(min_weight) of the map at the last
+ * update; changed_only = 1: the blocks of R, in (z, y, x) order, including blocks whose mesh is now empty (a viewer must learn that they
+ * lost their triangles).  Rejected: a call before any update, or after a clear / reset or a failed update with no successful update
+ * since.  One kernel launch when vertices are copied.
+ * ksg_mesh_view_device: the layer without a copy, in slot order: n_blocks slots, d_block_keys[slot] packed as ksg_device_map_view packs
+ * them, d_block_first[slot] .. d_block_first[slot + 1] the slot's vertices (n_blocks + 1 entries), d_rgba as r | g << 8 | b << 16 |
+ * a << 24.  Device memory owned by the integrator, valid until the next update, clear, reset or destroy; read it on the integrator's
+ * stream or after ksg_sync.  Refused as ksg_export_mesh is.  Every output pointer may be NULL. */
+typedef struct ksg_mesh_stats {
+  int64_t blocks;             /* allocated blocks the layer covers (= ksg_num_blocks) */
+  int64_t full;               /* 1: every block re-meshed (first call, new min_weight, after clear / reset / import, beyond the bound) */
+  int64_t changed_blocks;     /* |C| */
+  int64_t remeshed_blocks;    /* |R| */
+  int64_t vertices;           /* vertices in the layer now */
+  int64_t remeshed_vertices;  /* vertices emitted by this update */
+  int64_t reserved[4];
+} ksg_mesh_stats;
+int32_t ksg_update_mesh(ksg_integrator* h, float min_weight, ksg_mesh_stats* stats);
+int32_t ksg_export_mesh(ksg_integrator* h, int32_t changed_only, int64_t vertex_capacity, float* vertices, uint8_t* rgba, uint8_t* labels,
+                        int64_t block_capacity, int32_t* block_index, int64_t* block_first_vertex, int64_t* n_vertices, int64_t* n_blocks);
+int32_t ksg_mesh_view_device(ksg_integrator* h, int64_t* n_blocks, int64_t* n_vertices, const void** d_block_keys,
+                             const int64_t** d_block_first, const float** d_vertices, const uint32_t** d_rgba, const uint8_t** d_labels);
+
 /* Remove every block but keep the integrator: what Layer::removeAllBlocks() on both layers does to a live reference integrator.  The
  * fast integrator's two per-scan approximate sets (members of the integrator, fast.h:114-130) keep their contents and offsets, so the
  * next frame is integrated exactly as the reference integrator object would integrate it into its emptied layers.  Used by the

@@ -123,6 +123,23 @@ class KsgEsdfStats(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
 
 
+class KsgMeshStats(C.Structure):
+    """Mirror of `struct ksg_mesh_stats` (include/ksg.h): what one ksg_update_mesh re-meshed."""
+    _fields_ = [("blocks", C.c_int64), ("full", C.c_int64), ("changed_blocks", C.c_int64), ("remeshed_blocks", C.c_int64),
+                ("vertices", C.c_int64), ("remeshed_vertices", C.c_int64), ("reserved", C.c_int64 * 4)]
+
+    def as_dict(self) -> Dict[str, int]:
+        return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
+
+
+class _DeviceArray:
+    """A device pointer with a shape and a type string, as torch.as_tensor reads it (__cuda_array_interface__, no copy).  torch takes
+    no read-only arrays, so the caller must not write through the tensors of a view the library owns."""
+
+    def __init__(self, ptr: int, shape, typestr: str):
+        self.__cuda_array_interface__ = {"data": (int(ptr or 0), False), "shape": tuple(shape), "typestr": typestr, "version": 3}
+
+
 RENDER_FIELDS = ("depth", "points_G") + QUERY_FIELDS
 
 
@@ -317,6 +334,13 @@ def load_library(path: Optional[str] = None):
     lib.ksg_update_esdf.restype = C.c_int32
     lib.ksg_export_esdf.argtypes = [H, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.ksg_export_esdf.restype = C.c_int32
+    lib.ksg_update_mesh.argtypes = [H, C.c_float, C.POINTER(KsgMeshStats)]
+    lib.ksg_update_mesh.restype = C.c_int32
+    lib.ksg_export_mesh.argtypes = [H, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                    C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    lib.ksg_export_mesh.restype = C.c_int32
+    lib.ksg_mesh_view_device.argtypes = [H, C.POINTER(C.c_int64), C.POINTER(C.c_int64)] + [C.POINTER(C.c_void_p)] * 5
+    lib.ksg_mesh_view_device.restype = C.c_int32
     lib.ksg_query_esdf.argtypes = [H, C.c_int64, C.c_void_p, C.POINTER(KsgEsdfQueryOut)]
     lib.ksg_query_esdf.restype = C.c_int32
     lib.ksg_query_esdf_device.argtypes = [H, C.c_int64, C.c_void_p, C.POINTER(KsgEsdfQueryOut), C.c_void_p]
@@ -338,7 +362,8 @@ KSG_SYMBOLS = ["ksg_default_config", "ksg_create", "ksg_destroy", "ksg_last_erro
                "ksg_debug_chain_sum", "ksg_debug_tsdf_batch", "ksg_debug_apply_routes", "ksg_debug_fast_timeline", "ksg_integrate_depth_async", "ksg_wait_frame",
                "ksg_device_map_view", "ksg_merge_blocks_device", "ksg_copy_map_device", "ksg_integrate_image", "ksg_set_update_log", "ksg_fetch_update_log", "ksg_evaluate_labels", "ksg_extract_mesh", "ksg_clear_map", "ksg_copy_update_log_device", "ksg_merge_voxels_device",
                "ksg_query_points", "ksg_query_points_device", "ksg_render_view", "ksg_render_view_device", "ksg_compute_esdf",
-               "ksg_update_esdf", "ksg_export_esdf", "ksg_query_esdf", "ksg_query_esdf_device"]
+               "ksg_update_esdf", "ksg_export_esdf", "ksg_query_esdf", "ksg_query_esdf_device",
+               "ksg_update_mesh", "ksg_export_mesh", "ksg_mesh_view_device"]
 
 
 def debug_chain_sum(terms: np.ndarray, s0: float, lib=None) -> np.float32:
@@ -682,6 +707,39 @@ class Integrator:
                                               lab.ctypes.data_as(C.c_void_p), b, bidx.ctypes.data_as(C.c_void_p), first.ctypes.data_as(C.c_void_p),
                                               C.byref(nv), C.byref(nb)), "ksg_extract_mesh")
         return {"vertices": vtx, "rgba": rgba, "labels": lab, "block_index": bidx, "block_first": first}
+
+    def update_mesh(self, min_weight: float = 1e-4) -> Dict[str, int]:
+        """Bring the device mesh layer up to date with the map (ksg_update_mesh); returns its stats (KsgMeshStats fields)."""
+        st = KsgMeshStats()
+        self._check(self.lib.ksg_update_mesh(self.handle, min_weight, C.byref(st)), "ksg_update_mesh")
+        return st.as_dict()
+
+    def export_mesh(self, changed_only: bool = False):
+        """The device mesh layer as of the last update (ksg_export_mesh), in the layout of extract_mesh(): every block it covers, or with
+        changed_only the blocks the last update re-meshed (empty ones included), in (z, y, x) order."""
+        nv, nb = C.c_int64(), C.c_int64()
+        self._check(self.lib.ksg_export_mesh(self.handle, int(changed_only), 0, None, None, None, 0, None, None, C.byref(nv), C.byref(nb)),
+                    "ksg_export_mesh")
+        n, b = int(nv.value), int(nb.value)
+        vtx = np.zeros((n, 3), np.float32); rgba = np.zeros((n, 4), np.uint8); lab = np.zeros(n, np.uint8)
+        bidx = np.zeros((b, 3), np.int32); first = np.zeros(b + 1, np.int64)
+        self._check(self.lib.ksg_export_mesh(self.handle, int(changed_only), n, vtx.ctypes.data_as(C.c_void_p), rgba.ctypes.data_as(C.c_void_p),
+                                             lab.ctypes.data_as(C.c_void_p), b, bidx.ctypes.data_as(C.c_void_p),
+                                             first.ctypes.data_as(C.c_void_p), C.byref(nv), C.byref(nb)), "ksg_export_mesh")
+        return {"vertices": vtx, "rgba": rgba, "labels": lab, "block_index": bidx, "block_first": first}
+
+    def mesh_view_device(self):
+        """The device mesh layer without a copy (ksg_mesh_view_device), as torch tensors aliasing the integrator's memory (read them, never write), in slot order:
+        dict(block_keys [nb] i64 (packed), block_first [nb + 1] i64, vertices [n, 3] f32, rgba [n, 4] u8, labels [n] u8).  Valid until
+        the next update, clear, reset or close."""
+        import torch
+        nb, nv = C.c_int64(), C.c_int64()
+        p = [C.c_void_p() for _ in range(5)]
+        self._check(self.lib.ksg_mesh_view_device(self.handle, C.byref(nb), C.byref(nv), *(C.byref(x) for x in p)), "ksg_mesh_view_device")
+        b, n = int(nb.value), int(nv.value)
+        shapes = (((b,), "<i8"), ((b + 1,), "<i8"), ((n, 3), "<f4"), ((n, 4), "|u1"), ((n,), "|u1"))
+        names = ("block_keys", "block_first", "vertices", "rgba", "labels")
+        return {k: torch.as_tensor(_DeviceArray(x.value, shp, ts), device="cuda") for k, x, (shp, ts) in zip(names, p, shapes)}
 
     def esdf(self, max_distance: float, min_weight: float = 1e-4) -> Dict[str, np.ndarray]:
         """Batch Euclidean signed distance field of the map (ksg_compute_esdf): dict(block_index [nb, 3] i32 in export order,

@@ -36,6 +36,16 @@ class GpuIntegratorCore {
   // Semantic mesh of the device map (ksg_extract_mesh): triangle soup, per-vertex TsdfVoxel.color and semantic label, blocks in (z, y, x) order
   bool extractMesh(float min_weight, std::vector<float>* vertices, std::vector<uint8_t>* rgba, std::vector<uint8_t>* labels,
                    std::vector<int32_t>* block_index, std::vector<int64_t>* block_first);
+  // The semantic mesh kept on the device (ksg_update_mesh): re-meshes the blocks a change since the last call can reach, then returns,
+  // in extractMesh's layout, the meshes of the blocks that update re-meshed (ksg_export_mesh changed_only, blocks whose mesh is now
+  // empty included) - after a full update (first call, new min_weight, after a clear / reset / import, or after a call that failed)
+  // every block.  *full (may be NULL) tells which.  Works in kLazy mode without syncLayers().
+  bool updateMesh(float min_weight, std::vector<float>* vertices, std::vector<uint8_t>* rgba, std::vector<uint8_t>* labels,
+                  std::vector<int32_t>* block_index, std::vector<int64_t>* block_first, bool* full);
+  // The whole device mesh layer after bringing it up to date (ksg_update_mesh, then ksg_export_mesh of every block); the next
+  // updateMesh then returns every block.
+  bool meshLayer(float min_weight, std::vector<float>* vertices, std::vector<uint8_t>* rgba, std::vector<uint8_t>* labels,
+                 std::vector<int32_t>* block_index, std::vector<int64_t>* block_first);
   // Point queries on the device map (ksg_query_points), read-only and without a copy of the map: works in kLazy mode without
   // syncLayers().  Per point: flags (KSG_QUERY_*), the containing voxel (TsdfVoxel fields, SemanticVoxel label / log-probabilities /
   // colour; NaN / 0 when its block is not allocated), voxblox's trilinear distance and its gradient (NaN when not valid).
@@ -82,9 +92,12 @@ class GpuIntegratorCore {
 
  private:
   void copyBlocks(const std::vector<int32_t>& idx);
+  bool exportMesh(int32_t changed_only, std::vector<float>* vertices, std::vector<uint8_t>* rgba, std::vector<uint8_t>* labels,
+                  std::vector<int32_t>* block_index, std::vector<int64_t>* block_first);
   void syncAfterCall();        // eager mode: update log (fast) or updated blocks (merged)
   bool update_log_tried_ = false, update_log_on_ = false;
   bool esdf_resync_ = true;    // updateEsdf: the host layer must be refreshed whole (first call, or the last call failed)
+  bool mesh_resync_ = true;    // updateMesh: the caller must be given every block (first call, or the last call failed)
   ksg_integrator* handle_ = nullptr;
   vxb::Layer<vxb::TsdfVoxel>* tsdf_layer_;
   vxb::Layer<SemanticVoxel>* semantic_layer_;

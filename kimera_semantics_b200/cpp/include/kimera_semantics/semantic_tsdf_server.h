@@ -6,6 +6,7 @@
 #include <memory>
 #include <string>
 #include "kimera_semantics/map_io.h"
+#include "kimera_semantics/ply_io.h"
 #include "kimera_semantics/vxblx_io.h"
 #include "kimera_semantics/semantic_tsdf_integrator_factory.h"
 #include "kimera_semantics/semantic_tsdf_integrator_fast.h"
@@ -99,6 +100,21 @@ class SemanticTsdfServer {
   };
   bool extractMesh(SemanticMesh* mesh, float min_weight = 1e-4f) {
     return gpu().extractMesh(min_weight, &mesh->vertices, &mesh->rgba, &mesh->labels, &mesh->block_index, &mesh->block_first);
+  }
+  // voxblox's TsdfServer::updateMesh: brings the device mesh layer up to date with the map, re-meshing only the blocks a change since the
+  // last call can reach (GpuIntegratorCore::updateMesh, csrc/ksg_mesh.cuh), and returns in *changed the meshes of the blocks to publish:
+  // those re-meshed (a block whose mesh is now empty included: a viewer must drop its triangles), or after a full update every block
+  // (*full, may be NULL, says which).  A viewer keeps one mesh per block and replaces the blocks it is given.  Needs no updateLayers().
+  bool updateMesh(SemanticMesh* changed, float min_weight = 1e-4f, bool* full = nullptr) {
+    return gpu().updateMesh(min_weight, &changed->vertices, &changed->rgba, &changed->labels, &changed->block_index, &changed->block_first, full);
+  }
+  // voxblox's TsdfServer::generateMesh: the whole mesh layer, brought up to date as updateMesh does (GpuIntegratorCore::meshLayer),
+  // written to `ply_path` - the file the reference's `mesh_filename` parameter names - as the ASCII .ply of ply_io.h.  The next
+  // updateMesh returns every block.
+  bool generateMesh(const std::string& ply_path, float min_weight = 1e-4f) {
+    SemanticMesh mesh;
+    if (!gpu().meshLayer(min_weight, &mesh.vertices, &mesh.rgba, &mesh.labels, &mesh.block_index, &mesh.block_first)) return false;
+    return kimera_semantics::writeMeshPly(ply_path, mesh.vertices, mesh.rgba, mesh.labels);
   }
 
   // What a planner / scene-graph builder asks the map about points (Layer::getVoxelPtrByCoordinates + Interpolator::getDistance /

@@ -306,6 +306,35 @@ bool GpuIntegratorCore::extractMesh(float min_weight, std::vector<float>* vertic
   return ksg_extract_mesh(handle_, min_weight, nv, vertices->data(), rgba->data(), labels->data(), nb, block_index->data(), block_first->data(),
                           &nv, &nb) == KSG_OK;
 }
+bool GpuIntegratorCore::exportMesh(int32_t changed_only, std::vector<float>* vertices, std::vector<uint8_t>* rgba,
+                                   std::vector<uint8_t>* labels, std::vector<int32_t>* block_index, std::vector<int64_t>* block_first) {
+  int64_t nv = 0, nb = 0;
+  if (ksg_export_mesh(handle_, changed_only, 0, nullptr, nullptr, nullptr, 0, nullptr, nullptr, &nv, &nb) != KSG_OK) return false;
+  vertices->assign((size_t)nv * 3, 0.0f);
+  rgba->assign((size_t)nv * 4, 0);
+  labels->assign((size_t)nv, 0);
+  block_index->assign((size_t)nb * 3, 0);
+  block_first->assign((size_t)nb + 1, 0);
+  return ksg_export_mesh(handle_, changed_only, nv, vertices->data(), rgba->data(), labels->data(), nb, block_index->data(),
+                         block_first->data(), &nv, &nb) == KSG_OK;
+}
+bool GpuIntegratorCore::updateMesh(float min_weight, std::vector<float>* vertices, std::vector<uint8_t>* rgba, std::vector<uint8_t>* labels,
+                                   std::vector<int32_t>* block_index, std::vector<int64_t>* block_first, bool* full) {
+  const bool resync = mesh_resync_;
+  mesh_resync_ = true;
+  ksg_mesh_stats st;
+  if (ksg_update_mesh(handle_, min_weight, &st) != KSG_OK) return false;
+  const bool all = st.full || resync;
+  if (!exportMesh(all ? 0 : 1, vertices, rgba, labels, block_index, block_first)) return false;
+  if (full) *full = all;
+  mesh_resync_ = false;
+  return true;
+}
+bool GpuIntegratorCore::meshLayer(float min_weight, std::vector<float>* vertices, std::vector<uint8_t>* rgba, std::vector<uint8_t>* labels,
+                                  std::vector<int32_t>* block_index, std::vector<int64_t>* block_first) {
+  mesh_resync_ = true;   // this update's re-meshed blocks are not handed out: the next updateMesh returns every block
+  return ksg_update_mesh(handle_, min_weight, nullptr) == KSG_OK && exportMesh(0, vertices, rgba, labels, block_index, block_first);
+}
 
 bool GpuIntegratorCore::queryPoints(const vxb::Pointcloud& points_G, float min_weight, QueryResult* r) {
   static_assert(sizeof(vxb::Point) == 3 * sizeof(float), "points are passed as packed xyz triples");

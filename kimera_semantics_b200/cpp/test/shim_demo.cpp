@@ -1,7 +1,7 @@
 // Drives the drop-in C++ API exactly the way SemanticTsdfServer does (kimera_semantics_ros/src/semantic_tsdf_server.cpp:58-79):
 // build both layers, SemanticTsdfIntegratorFactory::create(method, ...), then integratePointCloud per frame.
 //   shim_demo <fast|merged|bogus> <frames.bin> <out.bin> [lazy] [--load ckpt] [--save ckpt] [--skip N] [--query in out] [--render in out]
-//             [--esdf max_distance out] [--esdf-every N max_distance out]
+//             [--esdf max_distance out] [--esdf-every N max_distance out] [--mesh-every N out.ply]
 //     --load: SemanticTsdfServer::loadMap before the first frame; --save: saveMap after the last; --skip: ignore the first N frames
 //     --depth file: instead of the clouds of frames.bin (whose frame count must then be 0) feed depth + label frames:
 //              int32 n, int32 width, int32 height, double K[4], then per frame float T[7], float depth[w*h], uint8 label[w*h]
@@ -16,11 +16,16 @@
 //              then vxblx_io::saveEsdfLayer to `out` - the reference driver's last step (kimera_semantics_rosbag.cpp:160-166)
 //     --esdf-every N max_distance out: SemanticTsdfServer::updateEsdf (min_weight 1e-4) into one host layer after every N-th frame of
 //              frames.bin and after the last, then vxblx_io::saveEsdfLayer of that layer to `out`
+//     --mesh-every N out.ply: SemanticTsdfServer::updateMesh (min_weight 1e-4) after every N-th frame of frames.bin and after the last,
+//              its blocks assembled into one host mesh (a viewer's copy: one mesh per block, replaced when a block comes back); that
+//              mesh must equal the final extractMesh; then SemanticTsdfServer::generateMesh writes `out.ply`
 // frames.bin : int32 n_frames, float voxel_size, int32 vps, int32 n_palette, palette n*(r,g,b,a,id), int32 n_dynamic, ids...,
 //              then per frame: int32 n, float T[7], float xyz[3n], uint8 rgba[4n]
 // out.bin    : int32 n_blocks, then per block (sorted z,y,x): int32 idx[3], per voxel: float d, float w, u8 rgba[4], u8 label,
 //              float priors[C], u8 sem_rgba[4]
 #include <algorithm>
+#include <array>
+#include <map>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -56,8 +61,8 @@ int main(int argc, char** argv) {
   const char *load_path = nullptr, *save_path = nullptr, *depth_path = nullptr, *query_in = nullptr, *query_out = nullptr;
   const char *render_in = nullptr, *render_out = nullptr, *esdf_out = nullptr;
   float esdf_max_distance = 0.0f, inc_max_distance = 0.0f;
-  const char* inc_out = nullptr;
-  int skip = 0, esdf_every = 0;
+  const char *inc_out = nullptr, *ply_out = nullptr;
+  int skip = 0, esdf_every = 0, mesh_every = 0;
   for (int a = 4; a < argc; ++a) {
     if (std::strcmp(argv[a], "lazy") == 0) lazy = true;
     else if (std::strcmp(argv[a], "--load") == 0 && a + 1 < argc) load_path = argv[++a];
@@ -71,6 +76,9 @@ int main(int argc, char** argv) {
       esdf_every = std::max(1, std::atoi(argv[++a]));
       inc_max_distance = (float)std::atof(argv[++a]);
       inc_out = argv[++a];
+    } else if (std::strcmp(argv[a], "--mesh-every") == 0 && a + 2 < argc) {
+      mesh_every = std::max(1, std::atoi(argv[++a]));
+      ply_out = argv[++a];
     }
   }
   SemanticTsdfServer::Params params;
@@ -84,7 +92,24 @@ int main(int argc, char** argv) {
   GpuIntegratorCore* core = &server.gpu();
   if (load_path) KSG_CHECK(server.loadMap(load_path)) << "cannot load " << load_path;
   vxb::Layer<vxb::EsdfVoxel> inc(tsdf_layer.voxel_size(), tsdf_layer.voxels_per_side());
-  int inc_updates = 0;
+  int inc_updates = 0, mesh_updates = 0;
+  // the viewer's copy of the mesh: block (x, y, z) -> its vertices, rgba and labels
+  std::map<std::array<int32_t, 3>, std::array<std::vector<uint8_t>, 3>> viewer;
+  auto publish = [&]() {
+    SemanticTsdfServer::SemanticMesh changed;
+    bool full = false;
+    KSG_CHECK(server.updateMesh(&changed, 1e-4f, &full)) << "mesh update failed";
+    if (full) viewer.clear();
+    for (size_t b = 0; b + 1 < changed.block_first.size(); ++b) {
+      const int64_t v0 = changed.block_first[b], v1 = changed.block_first[b + 1];
+      const auto* vb = reinterpret_cast<const uint8_t*>(changed.vertices.data());
+      std::array<std::vector<uint8_t>, 3>& m = viewer[{changed.block_index[3 * b], changed.block_index[3 * b + 1], changed.block_index[3 * b + 2]}];
+      m[0].assign(vb + 12 * v0, vb + 12 * v1);
+      m[1].assign(changed.rgba.begin() + 4 * v0, changed.rgba.begin() + 4 * v1);
+      m[2].assign(changed.labels.begin() + v0, changed.labels.begin() + v1);
+    }
+    ++mesh_updates;
+  };
   for (int fr = 0; fr < n_frames; ++fr) {
     const int n = rd<int32_t>(f);
     float T[7]; f.read(reinterpret_cast<char*>(T), sizeof(T));
@@ -99,6 +124,25 @@ int main(int argc, char** argv) {
       KSG_CHECK(server.updateEsdf(&inc, inc_max_distance)) << "esdf update failed";
       ++inc_updates;
     }
+    if (ply_out && (fr + 1) % mesh_every == 0) publish();
+  }
+  if (ply_out) {
+    publish();
+    SemanticTsdfServer::SemanticMesh want;
+    KSG_CHECK(server.extractMesh(&want)) << "mesh extraction failed";
+    std::array<std::vector<uint8_t>, 3> got;   // the viewer's blocks in (z, y, x) order, as extractMesh lists them
+    std::vector<std::array<int32_t, 3>> order;
+    for (const auto& kv : viewer) order.push_back(kv.first);
+    std::sort(order.begin(), order.end(), [](const std::array<int32_t, 3>& a, const std::array<int32_t, 3>& b) {
+      return a[2] != b[2] ? a[2] < b[2] : (a[1] != b[1] ? a[1] < b[1] : a[0] < b[0]); });
+    for (const auto& k : order)
+      for (int i = 0; i < 3; ++i) got[i].insert(got[i].end(), viewer[k][i].begin(), viewer[k][i].end());
+    const auto* wv = reinterpret_cast<const uint8_t*>(want.vertices.data());
+    const bool same = order.size() == want.block_index.size() / 3 && got[0] == std::vector<uint8_t>(wv, wv + 4 * want.vertices.size()) &&
+                      got[1] == want.rgba && got[2] == want.labels;
+    KSG_CHECK(server.generateMesh(ply_out)) << "cannot write " << ply_out;
+    std::printf("mesh-every: %d updates, assembled mesh %s extractMesh, %zu triangles\n", mesh_updates, same ? "equals" : "DIFFERS FROM",
+                want.vertices.size() / 9);
   }
   if (inc_out) {
     KSG_CHECK(server.updateEsdf(&inc, inc_max_distance)) << "esdf update failed";

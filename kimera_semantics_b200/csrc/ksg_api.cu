@@ -344,6 +344,22 @@ struct ksg_integrator {
   std::vector<uint8_t> esdf_has_site; // per slot: the row holds a site
   std::vector<int> esdf_rewritten;    // slots whose output the last update rewrote, in (z, y, x) order
 
+  // device mesh layer (ksg_update_mesh, ksg_mesh.cuh): per pool slot a vertex range of the arena, in slot order
+  unsigned* mesh_mark = nullptr;      // [max_blocks] 0 between updates
+  int *mesh_rpos = nullptr, *mesh_list = nullptr, *mesh_count = nullptr;   // [max_blocks]: list position of a marked slot, R, R's counts
+  long long* mesh_lfirst = nullptr;   // [max_blocks] first vertex of R's entries in the new arena
+  long long* mesh_first[2] = {nullptr, nullptr};   // [max_blocks + 1] per slot, of arena 0 / 1
+  MeshBuf mesh_arena[2] = {};
+  int64_t mesh_cap[2] = {0, 0};       // vertices each arena holds
+  MeshCounters *d_mesh_ctr = nullptr, *h_mesh_ctr = nullptr;   // h_: pinned
+  int mesh_cur = 0;                   // the arena of the layer
+  bool mesh_full = true;              // as esdf_full
+  bool mesh_valid = false;            // as esdf_valid: the layer describes slots [0, mesh_blocks)
+  bool mesh_far = false;              // a block of the layer lies beyond the window bound: every update is full
+  float mesh_min_weight = 0.0f;
+  int mesh_stamp = 0;
+  int64_t mesh_blocks = 0, mesh_vertices = 0, mesh_remeshed = 0;   // mesh_remeshed = |R| of the last update, listed in mesh_list
+
   long long* tile_debug = nullptr;  // optional per-tile (records, cycles) trace
   int apply_smem = 0;
   int apply_nch = 1;
@@ -423,6 +439,8 @@ int reset_map(ksg_integrator* h, cudaStream_t s) {
   h->merged_log_count = 0;
   h->esdf_full = true;
   h->esdf_valid = false;
+  h->mesh_full = true;
+  h->mesh_valid = false;
   KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
 }
@@ -1868,6 +1886,173 @@ int32_t ksg_extract_mesh(ksg_integrator* h, float min_weight, int64_t vertex_cap
   });
 }
 
+int32_t ksg_update_mesh(ksg_integrator* h, float min_weight, ksg_mesh_stats* stats) {
+  if (!h) return KSG_ERR_INVALID_ARGUMENT;
+  if (!(min_weight >= 0.0f)) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh update: NaN or negative min_weight");
+  if (h->dc.shard_count > 1) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh update: a sharded integrator holds only its own tiles");
+  { const int rcp = complete_frames(h); if (rcp) return rcp; }
+  const int64_t nb = h->num_blocks;
+  const bool full = h->mesh_full || h->mesh_far || min_weight != h->mesh_min_weight;
+  ksg_mesh_stats st{};
+  st.blocks = nb;
+  st.full = full ? 1 : 0;
+  if (!full && h->frame_stamp == h->mesh_stamp && nb == h->mesh_blocks) {   // nothing stamped, nothing allocated: no launch
+    st.vertices = h->mesh_vertices;
+    h->mesh_remeshed = 0;
+    if (stats) *stats = st;
+    return KSG_OK;
+  }
+  // Until this call succeeds the layer is not trusted: the marks and the arenas are rewritten in place.
+  h->mesh_full = true;
+  h->mesh_valid = false;
+  const int64_t prev = full ? 0 : h->mesh_blocks;   // slots below prev hold the meshes of the last update
+  const size_t rows = (size_t)h->map.max_blocks;
+  Resources& res = h->res;
+  if (!h->mesh_mark) {
+    KSG_CUDA(res.device(&h->mesh_mark, rows));
+    KSG_CUDA(res.device(&h->mesh_rpos, rows));
+    KSG_CUDA(res.device(&h->mesh_list, rows));
+    KSG_CUDA(res.device(&h->mesh_count, rows));
+    KSG_CUDA(res.device(&h->mesh_lfirst, rows));
+    KSG_CUDA(res.device(&h->mesh_first[0], rows + 1));
+    KSG_CUDA(res.device(&h->mesh_first[1], rows + 1));
+    KSG_CUDA(res.device(&h->d_mesh_ctr, 1));
+    KSG_CUDA(res.pinned(&h->h_mesh_ctr, 1));
+  }
+  cudaStream_t s = h->own_stream;
+  if (full) KSG_CUDA(cudaMemsetAsync(h->mesh_mark, 0, sizeof(unsigned) * rows, s));   // new, or left marked by a failed update
+  MeshCounters& ctr = *h->h_mesh_ctr;
+  std::memset(&ctr, 0, sizeof(ctr));
+  const int src = h->mesh_cur, dst = 1 - src;
+  if (nb > 0) {
+    KSG_CUDA(cudaMemsetAsync(h->d_mesh_ctr, 0, sizeof(MeshCounters), s));
+    const int64_t positions = (int64_t)h->ht_cap;
+    ++h->n_launches;
+    k_mesh_dirty<<<(int)std::min<int64_t>((positions + 255) / 256, (int64_t)h->sm_count * 8), 256, 0, s>>>(
+        h->map, (int)nb, (int)prev, h->mesh_stamp, h->dc.vps, h->mesh_mark, h->mesh_rpos, h->mesh_list, h->d_mesh_ctr);
+    KSG_CUDA(cudaMemcpyAsync(&ctr, h->d_mesh_ctr, sizeof(MeshCounters), cudaMemcpyDeviceToHost, s));
+    KSG_CUDA(cudaStreamSynchronize(s));
+    KSG_CUDA(cudaGetLastError());
+  }
+  const int nr = ctr.remeshed;
+  const int grid = (int)std::min<int64_t>(std::max(nr, 1), (int64_t)h->sm_count * 8);
+  if (nr > 0) {
+    const MeshBuf none{nullptr, nullptr, nullptr};
+    h->n_launches += 2;
+    k_mesh_blocks<false><<<grid, kMeshThreads, 0, s>>>(h->dc, h->map, h->mesh_list, nr, min_weight, nullptr, h->mesh_count, none);
+    k_mesh_scan<<<1, kMeshScanThreads, 0, s>>>((int)nb, h->mesh_mark, h->mesh_rpos, h->mesh_count, h->mesh_first[src], h->mesh_first[dst],
+                                               h->mesh_lfirst, h->d_mesh_ctr);
+    KSG_CUDA(cudaMemcpyAsync(&ctr.vertices, &h->d_mesh_ctr->vertices, 2 * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    KSG_CUDA(cudaStreamSynchronize(s));
+    KSG_CUDA(cudaGetLastError());
+    const int64_t total = ctr.vertices;
+    if (total > h->mesh_cap[dst]) {
+      MeshBuf& a = h->mesh_arena[dst];
+      const size_t want = (size_t)total + (size_t)total / 4;   // room to grow without a reallocation every update
+      int64_t c0 = 0, c1 = 0, c2 = 0;
+      h->mesh_cap[dst] = 0;
+      KSG_CUDA(res.regrow(&a.vtx, &c0, 3 * want));
+      KSG_CUDA(res.regrow(&a.rgba, &c1, want));
+      KSG_CUDA(res.regrow(&a.label, &c2, want));
+      h->mesh_cap[dst] = (int64_t)want;
+    }
+    h->n_launches += 2;
+    k_mesh_move<<<(int)std::min<int64_t>((nb + 7) / 8, (int64_t)h->sm_count * 16), 256, 0, s>>>(
+        (int)nb, nullptr, h->mesh_first[src], h->mesh_first[dst], 1, h->mesh_mark, h->mesh_arena[src], h->mesh_arena[dst]);
+    k_mesh_blocks<true><<<grid, kMeshThreads, 0, s>>>(h->dc, h->map, h->mesh_list, nr, min_weight, h->mesh_lfirst, nullptr, h->mesh_arena[dst]);
+    KSG_CUDA(cudaStreamSynchronize(s));
+    KSG_CUDA(cudaGetLastError());
+    h->mesh_cur = dst;
+  } else if (nb == 0) {
+    KSG_CUDA(cudaMemsetAsync(h->mesh_first[src], 0, sizeof(long long), s));   // first[0] = the total = 0
+    KSG_CUDA(cudaStreamSynchronize(s));
+  }
+  h->mesh_far = ctr.far != 0 || (!full && h->mesh_far);
+  h->mesh_full = false;
+  h->mesh_valid = true;
+  h->mesh_min_weight = min_weight;
+  h->mesh_stamp = h->frame_stamp;
+  h->mesh_blocks = nb;
+  h->mesh_vertices = nr > 0 ? ctr.vertices : h->mesh_vertices;
+  if (nb == 0) h->mesh_vertices = 0;
+  h->mesh_remeshed = nr;
+  st.changed_blocks = ctr.changed;
+  st.remeshed_blocks = nr;
+  st.vertices = h->mesh_vertices;
+  st.remeshed_vertices = nr > 0 ? ctr.remeshed_vertices : 0;
+  if (stats) *stats = st;
+  return KSG_OK;
+}
+
+int32_t ksg_export_mesh(ksg_integrator* h, int32_t changed_only, int64_t vertex_capacity, float* vertices, uint8_t* rgba, uint8_t* labels,
+                        int64_t block_capacity, int32_t* block_index, int64_t* block_first_vertex, int64_t* n_vertices, int64_t* n_blocks) {
+  if (!h || vertex_capacity < 0 || block_capacity < 0) return KSG_ERR_INVALID_ARGUMENT;
+  if (!h->mesh_valid) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh export: no ksg_update_mesh since the handle was created, cleared or reset");
+  KSG_CUDA(cudaSetDevice(h->device));
+  const int64_t nb = h->mesh_blocks;
+  // the blocks to list (slots), in (z, y, x) order, and the layer's per-slot first vertices
+  std::vector<uint64_t> keys((size_t)nb);
+  std::vector<long long> first((size_t)nb + 1, 0);
+  if (nb > 0) {
+    KSG_CUDA(cudaMemcpy(keys.data(), h->map.slot_key, sizeof(uint64_t) * nb, cudaMemcpyDeviceToHost));
+    KSG_CUDA(cudaMemcpy(first.data(), h->mesh_first[h->mesh_cur], sizeof(long long) * (nb + 1), cudaMemcpyDeviceToHost));
+  }
+  std::vector<int> list;
+  if (changed_only) {
+    list.resize((size_t)h->mesh_remeshed);
+    if (!list.empty()) KSG_CUDA(cudaMemcpy(list.data(), h->mesh_list, sizeof(int) * list.size(), cudaMemcpyDeviceToHost));
+    std::sort(list.begin(), list.end(), [&](int a, int b) { return keys[a] < keys[b]; });
+  } else {
+    list = zyx_order(keys);
+  }
+  const int64_t n = (int64_t)list.size();
+  std::vector<long long> out_first((size_t)n + 1);
+  out_first[0] = 0;
+  for (int64_t i = 0; i < n; ++i) out_first[i + 1] = out_first[i] + (first[list[i] + 1] - first[list[i]]);
+  const int64_t total = out_first[n];
+  if (n_blocks) *n_blocks = n;
+  if (n_vertices) *n_vertices = total;
+  if ((block_index || block_first_vertex) && n > block_capacity)
+    return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh export: block capacity too small (n_blocks holds the need)");
+  if (block_index) for (int64_t i = 0; i < n; ++i) put_block_index(block_index, i, keys[list[i]]);
+  if (block_first_vertex) for (int64_t i = 0; i <= n; ++i) block_first_vertex[i] = out_first[i];
+  if (!vertices && !rgba && !labels) return KSG_OK;                 // counting call
+  if (total > vertex_capacity) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh export: vertex capacity too small (n_vertices holds the need)");
+  if (total == 0) return KSG_OK;
+  HostStaging st;
+  const int* d_list = nullptr;
+  const long long* d_out_first = nullptr;
+  MeshBuf mb{};
+  st.in(&d_list, list.data(), (size_t)n);
+  st.in(&d_out_first, out_first.data(), (size_t)n);
+  st.out(&mb.vtx, vertices, 3 * (size_t)total, true);   // the kernel writes all three
+  st.out(&mb.rgba, reinterpret_cast<uint32_t*>(rgba), (size_t)total, true);
+  st.out(&mb.label, labels, (size_t)total, true);
+  cudaStream_t s = h->own_stream;
+  return st.run(h, s, [&] {
+    ++h->n_launches;
+    k_mesh_move<<<(int)std::min<int64_t>((n + 7) / 8, (int64_t)h->sm_count * 16), 256, 0, s>>>(
+        (int)n, d_list, h->mesh_first[h->mesh_cur], d_out_first, 0, nullptr, h->mesh_arena[h->mesh_cur], mb);
+    return KSG_OK;
+  });
+}
+
+int32_t ksg_mesh_view_device(ksg_integrator* h, int64_t* n_blocks, int64_t* n_vertices, const void** d_block_keys, const int64_t** d_block_first,
+                             const float** d_vertices, const uint32_t** d_rgba, const uint8_t** d_labels) {
+  if (!h) return KSG_ERR_INVALID_ARGUMENT;
+  if (!h->mesh_valid) return h->fail(KSG_ERR_INVALID_ARGUMENT, "mesh view: no ksg_update_mesh since the handle was created, cleared or reset");
+  static_assert(sizeof(long long) == sizeof(int64_t), "block_first layout");
+  const MeshBuf& a = h->mesh_arena[h->mesh_cur];
+  if (n_blocks) *n_blocks = h->mesh_blocks;
+  if (n_vertices) *n_vertices = h->mesh_vertices;
+  if (d_block_keys) *d_block_keys = h->map.slot_key;
+  if (d_block_first) *d_block_first = reinterpret_cast<const int64_t*>(h->mesh_first[h->mesh_cur]);
+  if (d_vertices) *d_vertices = a.vtx;
+  if (d_rgba) *d_rgba = a.rgba;
+  if (d_labels) *d_labels = a.label;
+  return KSG_OK;
+}
+
 namespace {
 bool query_wanted(const ksg_query_out& o) {
   return o.flags || o.tsdf_distance || o.tsdf_weight || o.tsdf_rgba || o.sem_label || o.sem_priors || o.sem_rgba || o.distance || o.gradient;
@@ -2472,6 +2657,7 @@ int32_t ksg_import_blocks(ksg_integrator* h, int64_t n, const int32_t* block_ind
   if (n == 0) return KSG_OK;
   { const int rcp = complete_frames(h); if (rcp) return rcp; }
   h->esdf_full = true;     // the import writes blocks without stamping them
+  h->mesh_full = true;
   const DevCfg& dc = h->dc;
   HostBlockTable table;
   { const int rct = table.load(h); if (rct) return rct; }
@@ -2823,6 +3009,8 @@ int32_t ksg_clear_map(ksg_integrator* h) {
   h->last_blocks_touched = 0;
   h->esdf_full = true;     // the stamps restart at 0 while frame_stamp does not, and the slots are reused
   h->esdf_valid = false;
+  h->mesh_full = true;
+  h->mesh_valid = false;
   KSG_CUDA(cudaStreamSynchronize(s));
   return KSG_OK;
 }
